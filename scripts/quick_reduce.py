@@ -1,4 +1,5 @@
 # scratch: device-resident timing of tg_reduce_by_key (Zipf s=1, U=2^26) with the per-kernel-class profile
+# usage: quick_reduce.py [n] [iters] [zipf|uniform] [sum_f64|min_f64|max_f64|sum_u64|min_u64|max_u64|first]
 import ctypes as C
 import os
 import sys
@@ -9,10 +10,11 @@ c = capi.Ctx(0)
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 125000000
 iters = int(sys.argv[2]) if len(sys.argv) > 2 else 5
 uniform = len(sys.argv) > 3 and sys.argv[3] == "uniform"
+op = sys.argv[4] if len(sys.argv) > 4 else "sum_f64"
 U = 1 << 26
 d_cdf = c.to_device(bench.zipf_cdf_numpy(U))
 d = c.alloc(n * 16)
-kvd = capi.KVDesc(16, capi.OP_SUM_F64)
+kvd = capi.KVDesc(16, getattr(capi, "OP_" + op.upper()))
 best = 1e9
 for i in range(iters):
     if uniform:
@@ -31,4 +33,4 @@ parts = []
 for k, nm in enumerate(names):
     t, cnt = c.profile_get(k)
     if cnt: parts.append("%s %.3f ms/%d" % (nm, t / cnt, cnt))
-print("reduce %s n=%d best %.3f ms = %.2f Grec/s distinct=%d | %s" % ("uniform" if uniform else "zipf", n, best, n / best / 1e6, rc.value, " | ".join(parts)), flush=True)
+print("reduce %s %s n=%d best %.3f ms = %.2f Grec/s distinct=%d | %s" % (op, "uniform" if uniform else "zipf", n, best, n / best / 1e6, rc.value, " | ".join(parts)), flush=True)

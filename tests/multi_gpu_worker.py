@@ -13,6 +13,7 @@ sys.path.insert(0, HERE)
 import torch.distributed as dist  # noqa: E402
 
 import oracle_lib as O  # noqa: E402
+import reduce_ref as RR  # noqa: E402
 import sort_ref as R  # noqa: E402
 from golden_util import golden, golden_r2, sha  # noqa: E402
 from gpu_util import make_blocks  # noqa: E402
@@ -183,6 +184,33 @@ def main():
         ref = O.reduce_simple(O.gen_reduce_zipf(0, nr * world, cdf, exact=1), O.OP_SUM_F64)
         assert np.array_equal(cat, ref), "large ReduceByKey differs from the oracle"
     tg.free(d); tg.free(d_cdf)
+
+    # ---- special values of one key split across the workers: the pre phase's partial aggregates of a key must fold into
+    # the contract's result in the post phase (reduce_ref.check), below and above the partitioned aggregation's threshold ----
+    inf, m0 = np.float64(np.inf).view(np.uint64), np.uint64(0x8000000000000000)
+    split = [(1, [m0] * 3),                                                      # -0.0 on every worker
+             (2, [m0] if rank == 0 else []),                                     # a lone -0.0 on one worker
+             (3, [np.uint64(RR.NAN_PAYLOADS[1])] if rank == 0 else list(np.array([rank, -rank], np.float64).view(np.uint64))),
+             (4, [np.uint64(RR.NAN_PAYLOADS[rank % len(RR.NAN_PAYLOADS)])]),     # NaN everywhere, payloads differ
+             (5, [inf] if rank == 0 else [inf ^ np.uint64(1 << 63)] if rank == world - 1 else [])]     # +inf and -inf
+    sk = np.concatenate([np.full(len(v), k, np.uint64) for k, v in split])
+    sv = np.array([x for _, v in split for x in v], dtype=np.uint64)
+    for nloc in (5000, 300000):
+        keys = np.random.default_rng(700 + rank).integers(1000, 1 << 40, size=nloc).astype(np.uint64)
+        for op, mix in (("sum_f64", "f64_special"), ("min_f64", "f64_special"), ("max_f64", "f64_special"), ("first", "u64"),
+                        ("sum_u64", "u64")):
+            kv = np.zeros(nloc + len(sk), dtype=O.KV)
+            kv["key"] = np.r_[keys, sk]
+            kv["val"] = np.r_[RR.gen_values(mix, keys, 900 + rank), sv]
+            d = tg.to_device(kv)
+            rp, rc = C.c_void_p(), C.c_size_t()
+            tg.ck(tg.L.tg_reduce_by_key(tg.h, C.byref(capi.KVDesc(16, RR.OPS.index(op))), d, len(kv), C.byref(rp), C.byref(rc)))
+            red = tg.download(rp.value, rc.value * 16, O.KV)
+            tg.free(d)
+            assert np.all(O.hash_partition_ids(red["key"], world) == rank), "key on the wrong worker"
+            ins, outs = gather(kv, world), gather(red, world)
+            if rank == 0:
+                RR.check(np.concatenate(ins), np.concatenate(outs), op)
 
     # ---- ReduceToIndex (PageRank step): the concatenation over the workers is the dense array of the reference ----
     cdf = O.zipf_cdf(1000)

@@ -26,8 +26,27 @@ using namespace tgp;
 namespace {
 
 // ---- the reduce functions the host shim recognises -----------------------------------------------------------
-__host__ inline bool op_identity_is_zero(int op) {
-    return op == TG_OP_SUM_F64 || op == TG_OP_SUM_U64 || op == TG_OP_MAX_U64 || op == TG_OP_FIRST;
+// Every table slot, accumulator and side slot starts at op_identity(op), and folding a key's first record into it must give
+// that record back bit for bit, as the reference stores a key's first record as is (core/reduce_probing_hash_table.hpp:201,
+// :251).  Sums of doubles start at -0.0 (-0.0 + x == x for every x, +0.0 + -0.0 == +0.0 would lose the sign), min/max of
+// doubles at a NaN that every value replaces (f64_better).  The identity of FIRST is never read.
+__host__ __device__ inline u64 op_identity(int op) {
+    switch (op) {
+    case TG_OP_SUM_F64: return 0x8000000000000000ull;          // -0.0
+    case TG_OP_MIN_U64: return ~0ull;
+    case TG_OP_MIN_F64:
+    case TG_OP_MAX_F64: return 0x7FF8000000000000ull;          // NaN
+    default: return 0ull;
+    }
+}
+
+// min/max of doubles (bit patterns): v replaces the accumulated o if it is smaller (larger), if o is the identity, or if o is
+// a NaN of the input and v a number.  A NaN never replaces a number, nor a NaN of the input, and the identity replaces
+// nothing: an accumulator that has seen a record holds one of the input's bit patterns, whatever unused accumulators
+// (still the identity) are folded into it.
+__device__ __forceinline__ bool f64_better(int op, u64 vb, u64 ob) {
+    const double v = __longlong_as_double((long long)vb), o = __longlong_as_double((long long)ob);
+    return (op == TG_OP_MIN_F64 ? v < o : o < v) || (isnan(o) && (!isnan(v) || ob == op_identity(op)));
 }
 
 // atomically fold `val` into *slot_val; `claimed` = this thread created the slot (needed for FIRST)
@@ -39,12 +58,9 @@ __device__ __forceinline__ void op_apply(int op, u64* slot_val, u64 val, bool cl
     case TG_OP_MAX_U64: atomicMax(slot_val, val); break;
     case TG_OP_MIN_F64:
     case TG_OP_MAX_F64: {
-        double v = __longlong_as_double((long long)val);
         u64 old = *(volatile u64*)slot_val;
         while (true) {
-            double o = __longlong_as_double((long long)old);
-            bool better = (op == TG_OP_MIN_F64) ? (v < o) : (o < v);
-            if (!better) break;
+            if (!f64_better(op, val, old)) break;
             u64 prev = atomicCAS(slot_val, old, val);
             if (prev == old) break;
             old = prev;
@@ -177,9 +193,7 @@ int get_scratch(tg_ctx* ctx, int op, ReduceScratch* sc) {
     sc->cursor = d + 4096;
     sc->zero_slot = d + 4100;
     u64 init[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
-    u64 ident = (op == TG_OP_MIN_U64) ? ~0ull : (op == TG_OP_MIN_F64) ? 0x7FF0000000000000ull
-              : (op == TG_OP_MAX_F64) ? 0xFFF0000000000000ull : 0ull;
-    init[5] = ident;        // zero_slot[1]
+    init[5] = op_identity(op);        // zero_slot[1]
     u64* h = (u64*)ctx->pinned + 1024;
     memcpy(h, init, sizeof(init));
     TG_CUDA(ctx, cudaMemcpyAsync(sc->cursor, h, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
@@ -202,11 +216,9 @@ int run_aggregate(tg_ctx* ctx, int op, const void* d_in, u64 m, void* d_out, u64
     u64 cap = m + m / 2 + 64;                     // load factor <= 2/3
     ulonglong2* tab;
     TG_TRY(tg_ws_get(ctx, WS_TABLE, cap * 16, (void**)&tab));
-    if (op_identity_is_zero(op)) TG_CUDA(ctx, cudaMemsetAsync(tab, 0, cap * 16, ctx->stream));
-    else {
-        u64 ident = (op == TG_OP_MIN_U64) ? ~0ull : (op == TG_OP_MIN_F64) ? 0x7FF0000000000000ull : 0xFFF0000000000000ull;
-        TG_LAUNCH(ctx, table_init_kernel, ctx->sm_count * 8, 512, 0, tab, cap, ident);
-    }
+    const u64 ident = op_identity(op);
+    if (ident == 0) TG_CUDA(ctx, cudaMemsetAsync(tab, 0, cap * 16, ctx->stream));
+    else TG_LAUNCH(ctx, table_init_kernel, ctx->sm_count * 8, 512, 0, tab, cap, ident);
     TG_LAUNCH_T(ctx, TG_K_AGGREGATE, aggregate_kernel, ctx->sm_count * 4, 512, 0, (const ulonglong2*)d_in, m, op, tab, cap, sc.zero_slot);
     TG_LAUNCH_T(ctx, TG_K_COMPACT, compact_kernel, ctx->sm_count * 4, 512, 0, (const ulonglong2*)tab, cap, (ulonglong2*)d_out, sc.cursor, sc.zero_slot);
     return read_cursor(ctx, sc, out_distinct);
@@ -247,8 +259,8 @@ __device__ __forceinline__ u64 op_combine(int op, u64 a, u64 b) {
     case TG_OP_SUM_U64: return a + b;
     case TG_OP_MIN_U64: return a < b ? a : b;
     case TG_OP_MAX_U64: return a > b ? a : b;
-    case TG_OP_MIN_F64: return __longlong_as_double((long long)b) < __longlong_as_double((long long)a) ? b : a;
-    case TG_OP_MAX_F64: return __longlong_as_double((long long)a) < __longlong_as_double((long long)b) ? b : a;
+    case TG_OP_MIN_F64:
+    case TG_OP_MAX_F64: return f64_better(op, b, a) ? b : a;
     default: return a;          // TG_OP_FIRST
     }
 }
@@ -694,8 +706,7 @@ bool reduce_unstable() {
 // n records -> distinct keys in d_out (capacity n + 1)
 int run_partitioned_aggregate(tg_ctx* ctx, int op, const void* d_in, u64 n, void* d_out, u64* out_distinct) {
     if (n < AGG_MIN_ITEMS || n >= (1u << 30) || getenv("TG_REDUCE_HBM_TABLE")) return run_aggregate(ctx, op, d_in, n, d_out, out_distinct);
-    const u64 ident = (op == TG_OP_MIN_U64) ? ~0ull : (op == TG_OP_MIN_F64) ? 0x7FF0000000000000ull
-                    : (op == TG_OP_MAX_F64) ? 0xFFF0000000000000ull : 0ull;
+    const u64 ident = op_identity(op);
     void *bufA, *bufB;
     TG_TRY(tg_ws_get(ctx, WS_AUX, (n + 2) * 16, &bufA));
     TG_TRY(tg_ws_get(ctx, WS_AUX2, (n + 2) * 16, &bufB));
