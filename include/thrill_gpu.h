@@ -14,6 +14,12 @@
  * per ctx.  Collective entry points (tg_sort, tg_reduce_by_key with nranks > 1) must be entered by all
  * ranks in the same order — the rule Thrill has for GetNewMixStream (api/context.hpp:308-316).
  * Device buffers passed in must be 16-byte aligned.  There is NO CPU fallback anywhere behind this ABI.
+ *
+ * Limits (TG_ERR_TOO_LARGE, checked before any work): every entry point that takes a device item count (tg_radix_sort_local,
+ * tg_classify_scatter, tg_hash_aggregate, tg_hash_partition, tg_sort, tg_reduce_by_key, tg_reduce_to_index and their
+ * _file / _dev forms) takes at most 2^30 - 1 items per call and worker (n_local), and a worker receives at most 2^30 - 1
+ * items in an exchange: the partition passes count in 30-bit fields.  ReduceToIndex gives each worker fewer than 2^31
+ * indices of the result.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
  ******************************************************************************/
 #ifndef THRILL_GPU_H
 #define THRILL_GPU_H
@@ -32,7 +38,7 @@ typedef enum {
     TG_ERR_CUDA = -1,          /* a CUDA runtime call failed */
     TG_ERR_NCCL = -2,          /* an NCCL call failed */
     TG_ERR_ARG = -3,           /* bad argument / unsupported descriptor */
-    TG_ERR_TOO_LARGE = -4,     /* n exceeds the per-call limit (2^30 - 1 items per GPU) */
+    TG_ERR_TOO_LARGE = -4,     /* over a per-call limit (see Limits above) */
     TG_ERR_NO_DEVICE = -5,     /* no sm_90 device: the product path fails loudly, never falls back */
     TG_ERR_OOM = -6
 } tg_status;
@@ -210,8 +216,7 @@ int tg_exchange_plan(uint32_t p, uint32_t me, const uint32_t* counts, uint64_t* 
  * of what was received.  d_in holds n_local items (it is clobbered); *out_dptr points to *out_n items inside a ctx-owned
  * workspace, the exchange window or d_in itself: valid until the next operator call on this ctx, never to be freed by the
  * caller (tg_free rejects it), to be copied (or detached with tg_output_detach after a *_file / *_dev call) before it is
- * fed to another operator.  Limits: n_local < 2^30, at most 16 ranks.  Collective: sizes are agreed on by all ranks,
- * TG_ERR_TOO_LARGE is returned by every rank or by none. */
+ * fed to another operator.  At most 16 ranks.  Collective: sizes are agreed on by all ranks. */
 int tg_sort(tg_ctx* ctx, const tg_key_desc* desc, void* d_in, size_t n_local, uint64_t rng_seed,
             void** out_dptr, size_t* out_n);
 

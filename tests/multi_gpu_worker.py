@@ -222,6 +222,33 @@ def main():
     parts = gather(red.items, world)
     if rank == 0:
         assert np.array_equal(np.concatenate(parts), g["reduce_to_index_zipf_u1000_20000_exact1_w3"]), "ReduceToIndex differs from the reference"
+
+    # ---- the item limit: one worker holds 2^30 records (a real buffer), the others a few; every rank gets TG_ERR_TOO_LARGE
+    # and nobody is left waiting in a collective.  Then the ctx still reduces. ----
+    big = rank == world - 1
+    n_local = (1 << 30) if big else 1000
+    d = tg.alloc(n_local * 16)
+    tg.upload(d, np.zeros(2 * min(n_local, 1000), dtype=np.uint64))
+    kvd = capi.KVDesc(16, capi.OP_SUM_U64)
+    rp, rc, rb = C.c_void_p(), C.c_size_t(), C.c_uint64()
+    neutral = np.zeros(2, dtype=np.uint64)
+    for name, call in (("reduce_by_key", lambda: tg.L.tg_reduce_by_key(tg.h, C.byref(kvd), d, n_local, C.byref(rp), C.byref(rc))),
+                       ("reduce_to_index", lambda: tg.L.tg_reduce_to_index(tg.h, C.byref(kvd), d, n_local, 1 << 20, neutral.ctypes.data,
+                                                                           C.byref(rp), C.byref(rc), C.byref(rb)))):
+        st = call()
+        assert st == -4, "%s: rank %d (n_local %d) returned %d, expected TG_ERR_TOO_LARGE on every rank" % (name, rank, n_local, st)
+    tg.free(d)
+    kv = np.zeros(1000, dtype=O.KV)
+    kv["key"] = np.arange(1000) % 7
+    kv["val"] = 1
+    d = tg.to_device(kv)
+    tg.ck(tg.L.tg_reduce_by_key(tg.h, C.byref(kvd), d, len(kv), C.byref(rp), C.byref(rc)))
+    red = tg.download(rp.value, rc.value * 16, O.KV)
+    tg.free(d)
+    outs = gather(red, world)
+    if rank == 0:
+        cat = np.concatenate(outs)
+        assert np.array_equal(np.sort(cat["key"]), np.arange(7)) and int(cat["val"].sum()) == 1000 * world
     dist.barrier()
     ctx.close()
     if rank == 0:

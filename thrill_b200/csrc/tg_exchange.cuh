@@ -36,12 +36,15 @@ int xchg_upload_dest(tg_ctx* ctx, int item_bytes, const XchgResult& res, void***
 void xchg_recv_offsets(tg_ctx* ctx, u64* before);                  // before[d] = items of the lower ranks in worker d's window
 
 // Stable partition of n local items by fn (destination worker, < p) + Alltoallv.  Collective.
+// n >= 2^30 (over the per-call limit): this rank sends nothing and reports 2^30 items for worker 0 in its counts, so that
+// xchg_counts returns TG_ERR_TOO_LARGE on every rank and none is left waiting in a collective.
 template <int WORDS, class DigitFn>
 int exchange_scatter(tg_ctx* ctx, const void* d_in, size_t n, const DigitFn& fn, XchgResult* res) {
     typedef typename ItemT<WORDS>::type Item;
     const int p = ctx->nranks;
     const size_t s = sizeof(Item);
-    if (n >= (1u << 30)) n = 0;              // (the caller has validated n on every rank before the first collective)
+    const bool too_large = n >= (1u << 30);
+    if (too_large) n = 0;
     TG_TRY(xwin_negotiate(ctx));
     // (1) destination histogram per chunk
     const ChunkGeom g = chunk_geometry<WORDS>(ctx, n);
@@ -57,6 +60,7 @@ int exchange_scatter(tg_ctx* ctx, const void* d_in, size_t n, const DigitFn& fn,
         TG_LAUNCH(ctx, chunk_scan_kernel, 1, 4 * RADIX, 0, chunkcount, g.nchunks, totals, totals + RADIX, chunkbase);
     }
     else TG_CUDA(ctx, cudaMemsetAsync(totals, 0, 2 * RADIX * 4, ctx->stream));
+    if (too_large) TG_CUDA(ctx, cudaMemsetAsync((char*)totals + 3, 0x40, 1, ctx->stream));     // totals[0] = 0x40000000 = 2^30
     // (2) count matrix; every rank learns every rank's receive size
     u64 need = 0;
     TG_TRY(xchg_counts(ctx, totals, (int)s, res, &need));

@@ -898,6 +898,7 @@ extern "C" {
 
 int tg_hash_aggregate(tg_ctx* ctx, const tg_kv_desc* desc, const void* d_in, size_t n, void* d_out, uint64_t* out_distinct) {
     TG_TRY(check_kv(ctx, desc));
+    if (n >= (1u << 30)) return tg_set_error(ctx, TG_ERR_TOO_LARGE, "hash_aggregate: n=%zu", n);
     TG_CUDA(ctx, cudaSetDevice(ctx->device));
     u64 distinct = 0;
     TG_TRY(run_partitioned_aggregate(ctx, (int)desc->op, d_in, n, d_out, &distinct));
@@ -926,12 +927,17 @@ int tg_reduce_by_key(tg_ctx* ctx, const tg_kv_desc* desc, const void* d_in, size
     TG_CUDA(ctx, cudaSetDevice(ctx->device));
     const int op = (int)desc->op;
     const int p = ctx->nranks, me = ctx->rank;
+    // n_local >= 2^30: with several workers, the exchange reports it to every rank (a uniform TG_ERR_TOO_LARGE)
+    const bool too_large = n_local >= (1u << 30);
+    if (too_large && p == 1) return tg_set_error(ctx, TG_ERR_TOO_LARGE, "reduce_by_key: n_local=%zu", n_local);
     // pre phase (ReducePrePhase, StartPreOp..StopPreOp: api/reduce_by_key.hpp:142-168): the local aggregation; with one
     // worker it is already the result
-    void* d_pre;
-    TG_TRY(tg_ws_get(ctx, WS_OUT, (n_local + 2) * 16, &d_pre));
-    u64 m = 0;
-    TG_TRY(run_partitioned_aggregate(ctx, op, d_in, n_local, d_pre, &m));
+    void* d_pre = nullptr;
+    u64 m = n_local;
+    if (!too_large) {
+        TG_TRY(tg_ws_get(ctx, WS_OUT, (n_local + 2) * 16, &d_pre));
+        TG_TRY(run_partitioned_aggregate(ctx, op, d_in, n_local, d_pre, &m));
+    }
     if (p == 1) {
         *out_dptr = d_pre;
         *out_n = (size_t)m;
@@ -961,15 +967,23 @@ int tg_reduce_to_index(tg_ctx* ctx, const tg_kv_desc* desc, const void* d_in, si
     TG_CUDA(ctx, cudaSetDevice(ctx->device));
     const int op = (int)desc->op;
     const int p = ctx->nranks, me = ctx->rank;
-    // the index range of this worker: Range(0, size).Partition(me, p) (common/math.hpp:85-94)
-    const u64 begin = ((u64)me * result_size + p - 1) / p, end = ((u64)(me + 1) * result_size + p - 1) / p;
-    const u64 count = end - begin;
-    if (count >= (1ull << 31)) return tg_set_error(ctx, TG_ERR_TOO_LARGE, "reduce_to_index: %llu indices per worker", (unsigned long long)count);
+    // the index range of this worker: Range(0, size).Partition(me, p) (common/math.hpp:85-94).  The limit is checked on the
+    // largest range of any worker, so that every rank returns the same verdict.
+    auto range_begin = [&](u64 r) { return (u64)(((unsigned __int128)r * result_size + p - 1) / p); };
+    const u64 begin = range_begin(me), count = range_begin(me + 1) - begin;
+    u64 max_count = 0;
+    for (int r = 0; r < p; ++r) max_count = std::max(max_count, range_begin(r + 1) - range_begin(r));
+    if (max_count >= (1ull << 31)) return tg_set_error(ctx, TG_ERR_TOO_LARGE, "reduce_to_index: %llu indices per worker", (unsigned long long)max_count);
+    // n_local >= 2^30: with several workers, the exchange reports it to every rank (a uniform TG_ERR_TOO_LARGE)
+    const bool too_large = n_local >= (1u << 30);
+    if (too_large && p == 1) return tg_set_error(ctx, TG_ERR_TOO_LARGE, "reduce_to_index: n_local=%zu", n_local);
     // pre phase: local aggregation by index
-    void* d_pre;
-    TG_TRY(tg_ws_get(ctx, WS_OUT, (n_local + 2) * 16, &d_pre));
-    u64 m = 0;
-    TG_TRY(run_partitioned_aggregate(ctx, op, d_in, n_local, d_pre, &m));
+    void* d_pre = nullptr;
+    u64 m = n_local;
+    if (!too_large) {
+        TG_TRY(tg_ws_get(ctx, WS_OUT, (n_local + 2) * 16, &d_pre));
+        TG_TRY(run_partitioned_aggregate(ctx, op, d_in, n_local, d_pre, &m));
+    }
     const void* d_post = d_pre;
     u64 m_post = m;
     if (p > 1) {
