@@ -22,6 +22,6 @@ for i in range(iters):
 pm, pc = c.profile_get(capi.K_PARTITION); hm, hc = c.profile_get(capi.K_RADIX_HIST)
 fm, fc = c.profile_get(capi.K_FIXUP); sm, sc = c.profile_get(capi.K_SEGCOUNT)
 ok = c.is_sorted(desc, d, n) and c.checksum(d, n, 8) == cs0
-print("cfg=%s n=%d best %.3f ms = %.2f Gkeys/s | partition %.4f ms/launch (%d) = %.0f GB/s | hist %.4f ms | fixup %.4f ms (%d) | segcount %.4f ms (%d) | correct=%s"
-      % (os.environ.get("TG_SWEEP_CFG", "0"), n, best, n / best / 1e6, pm / max(pc, 1), pc,
+print("n=%d best %.3f ms = %.2f Gkeys/s | partition %.4f ms/launch (%d) = %.0f GB/s | hist %.4f ms | fixup %.4f ms (%d) | segcount %.4f ms (%d) | correct=%s"
+      % (n, best, n / best / 1e6, pm / max(pc, 1), pc,
          16 * n / (pm / max(pc, 1)) / 1e6, hm / max(hc, 1), fm / max(fc, 1), fc, sm / max(sc, 1), sc, ok), flush=True)

@@ -7,7 +7,7 @@ import ctypes as C
 import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("TG_LIB") or os.path.join(HERE, "csrc", "libthrill_gpu.so")      # TG_LIB: experiment builds (scripts/build_variant.sh)
+LIB_PATH = os.environ.get("TG_LIB") or os.path.join(HERE, "csrc", "libthrill_gpu.so")      # TG_LIB: another build of the library, e.g. for an A/B comparison
 
 TG_OK = 0
 KEY_UINT_LE, KEY_BYTES_BE = 0, 1

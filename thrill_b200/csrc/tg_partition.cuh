@@ -3,7 +3,7 @@
 //   * the splitter classify/scatter (digit = destination worker by the splitters)   tg_sample_sort.cu
 //   * the hash aggregation          (digit = a byte of Hash128to64(0,key), or % p)  tg_reduce.cu
 //
-// Persistent CTAs walk a list of tiles in static round-robin order.  A tile (32-64 KB) is staged into shared memory by
+// Persistent CTAs walk a list of tiles in static round-robin order.  A tile (64 KB) is staged into shared memory by
 // the TMA unit (cp.async.bulk + mbarrier, double buffered: the next tile lands while the current one is processed), ranked
 // stably with warp-synchronous ballots + warp-private counters, positioned by a chained scan with batched decoupled
 // look-back over the tiles of its SEGMENT (the whole input for the plain pass; see tg_segmented.cuh for the chunked and
@@ -11,24 +11,9 @@
 // (re-used) landing buffer and written out so that consecutive threads write consecutive addresses.
 // HBM traffic: read n*s + write n*s + ~3 % scan state.
 #pragma once
-#include <stdlib.h>
-
 #include "tg_common.cuh"
 
 namespace tgp {
-
-#ifndef TG_LB
-#define TG_LB 8
-#endif
-#ifndef TG_PF
-#define TG_PF 1
-#endif
-#ifndef TG_MATCH_MIX
-#define TG_MATCH_MIX 0   // 1: experiment, see rank_rows
-#endif
-#ifndef TG_LB_SEG
-#define TG_LB_SEG 8      // (a dominant segment's tiles still run concurrently at the tail of the list: keep the batch deep)
-#endif
 
 constexpr int RADIX_BITS = 8;
 constexpr int RADIX = 1 << RADIX_BITS;
@@ -102,21 +87,23 @@ __device__ __forceinline__ u32 match_digit8(u32 d) {
     return peers;
 }
 
-// tile geometry of one launch configuration: THREADS threads, each owning IPT items of WORDS 8-byte words
+// Launch configuration of the partition pass: 512 threads per CTA, each owning 16 8-byte words (16 u64 items or 8 16-byte
+// items), one CTA per SM.  On H100 this was the fastest of the configurations measured for 8- and 16-byte items (see
+// DESIGN.md §5).  Tile sizes: 8192 items of 8 bytes, 4096 of 16 bytes.
 constexpr int PEER_MAX = 32;        // destinations of a partition pass that stores into peer windows (<= TG_MAX_RANKS used)
-template <int WORDS, int THREADS, int IPT, bool TMA = true, bool STORE = true, bool PEER = false, int SCRATCH = 0>
-struct SweepCfg {
+template <int WORDS, bool STORE = true, bool PEER = false, int SCRATCH = 0>
+struct PartCfg {
+    static constexpr int THREADS = 512;
+    static constexpr int MIN_BLOCKS = 1;                     // CTAs per SM
     static constexpr int ITEM_BYTES = 8 * WORDS;
-    static constexpr int ITEMS = IPT;
+    static constexpr int ITEMS = 16 / WORDS;                 // items per thread
     static constexpr int TILE = THREADS * ITEMS;             // items per tile
     static constexpr int TILE_BYTES = TILE * ITEM_BYTES;
     static constexpr int NWARPS = THREADS / 32;
-    // 2 landing/exchange buffers | warp counters [NWARPS][RADIX] | goff [RADIX] | warp_tot [16] | mbar [2] | dig [TILE]
     static constexpr int BUF_BYTES = TILE_BYTES + (WORDS == 1 ? 16 : 0);      // + one 16-byte granule: tiles that start at an odd 8-byte item
-    static constexpr int NBUF = TMA ? 2 : 1;                // landing + exchange, or the exchange buffer alone
-    // buffers | warp counters [NWARPS][RADIX] | goff [RADIX] | warp_tot [16] | mbar [2] | digit bytes [TILE] (only if the digit
-    // function's result is kept, kStoreDigit) | slack
-    static constexpr int SMEM = NBUF * BUF_BYTES + NWARPS * RADIX * (int)sizeof(unsigned short) + RADIX * 4 + 64 + 16 + (STORE ? TILE : 0) + (PEER ? PEER_MAX * 8 : 0) + SCRATCH + 128;
+    // 2 landing/exchange buffers | warp counters [NWARPS][RADIX] | goff [RADIX] | warp_tot [16] | mbar [2] | digit bytes [TILE]
+    // (only if the digit function's result is kept, kStoreDigit) | peer pointers [PEER_MAX] | functor scratch | slack
+    static constexpr int SMEM = 2 * BUF_BYTES + NWARPS * RADIX * (int)sizeof(unsigned short) + RADIX * 4 + 64 + 16 + (STORE ? TILE : 0) + (PEER ? PEER_MAX * 8 : 0) + SCRATCH + 128;
 };
 
 // exclusive scan of npass digit histograms -> global bases; skip[p] = 1 if one bin holds everything
@@ -149,8 +136,7 @@ __device__ __forceinline__ u32 lds_u32(u32 addr) {
     return v;
 }
 __device__ __forceinline__ void sts_u32(u32 addr, u32 v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
-// the warp-private digit counters are 16-bit (a tile holds < 65536 items): half the shared memory, which is what lets a third
-// CTA of the 16-byte-item configuration fit on an SM
+// the warp-private digit counters are 16-bit (a tile holds < 65536 items): half the shared memory of 32-bit counters
 typedef unsigned short cnt_t;
 __device__ __forceinline__ u32 lds_cnt(u32 addr) {
     u32 v;
@@ -164,7 +150,7 @@ __device__ __forceinline__ void sts_cnt(u32 addr, u32 v) { asm volatile("st.shar
 // address of the warp's RADIX counters.  rank = position inside the group | digit << 16 (if STORE).
 template <bool FULL, bool STORE, int ITEMS, class Item, class DigitFn>
 __device__ __forceinline__ void rank_rows(const Item (&key)[ITEMS], u32 (&rank)[ITEMS], const DigitFn& fn, u32 whist_w,
-                                          u32 pos0, u32 tile_base, u32 tile_valid, u32 lt, bool nomatch = false) {
+                                          u32 pos0, u32 tile_base, u32 tile_valid, u32 lt) {
 #pragma unroll
     for (int i = 0; i < ITEMS; ++i) {
         const u32 p = pos0 + i * 32;
@@ -172,12 +158,7 @@ __device__ __forceinline__ void rank_rows(const Item (&key)[ITEMS], u32 (&rank)[
         if (!FULL && p >= tile_valid) d = RADIX - 1;
         const u32 a = whist_w + d * (u32)sizeof(cnt_t);
         const u32 old = lds_cnt(a);
-#if TG_MATCH_MIX
-        // experiment build (scripts/build_variant.sh "-DTG_MATCH_MIX=1"): every other row on the ADU pipe (match.any.sync)
-        const u32 peers = nomatch ? (~lt & (lt << 1 | 1u)) : ((i & 1) ? __match_any_sync(0xffffffffu, d) : match_digit8(d));
-#else
-        const u32 peers = nomatch ? (~lt & (lt << 1 | 1u)) : match_digit8(d);
-#endif
+        const u32 peers = match_digit8(d);
         const u32 below = peers & lt;
         if (below == 0) sts_cnt(a, old + __popc(peers));
         rank[i] = old + __popc(below);
@@ -225,30 +206,25 @@ __device__ __forceinline__ u32 seg_num_tiles(const SegList& sl) { return sl.num_
 // PEER: the buckets are destination workers; bucket d is written to dbase[d][position], where dbase[d] points into worker
 // d's exchange window (mapped peer memory: the stores travel over NVLink) biased so that `position` is the position the
 // plain pass would have used in `out` — the Alltoallv of the reference's MixStream exchange happens inside the pass.
-template <int WORDS, int THREADS, int IPT, int MINB, class DigitFn, bool SEG, bool DBG = false, bool TMA = true, bool PEER = false,
-          bool UNSTABLE = false>
-__global__ void __launch_bounds__(THREADS, MINB)
+template <int WORDS, class DigitFn, bool SEG, bool PEER, bool UNSTABLE>
+__global__ void __launch_bounds__(PartCfg<WORDS>::THREADS, PartCfg<WORDS>::MIN_BLOCKS)
 partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename ItemT<WORDS>::type* __restrict__ out,
                  u32 n, const DigitFn fn_param, const u32* __restrict__ gbase, u32* __restrict__ status, const SegList sl,
-                 int dbg, typename ItemT<WORDS>::type* const* __restrict__ dbase) {
-    // DBG instantiations (TG_SWEEP_DEBUG, timing experiments only, results are wrong): dbg bit0 = no look-back wait,
-    // bit1 = no matching, bit2 = linear instead of scattered write-out, bit3 = no write-out
+                 typename ItemT<WORDS>::type* const* __restrict__ dbase) {
     typedef typename ItemT<WORDS>::type Item;
-    // TMA = false: no landing buffer and no bulk copies; the items are loaded straight into registers (coalesced 8/16-byte
-    // loads) and several small CTAs per SM hide each other's load latency and barriers instead of the double buffer
-    typedef SweepCfg<WORDS, THREADS, IPT, TMA, DigitFn::kStoreDigit, PEER, DigitFn::kScratch> C;
-    constexpr int ITEMS = C::ITEMS, TILE = C::TILE, NWARPS = C::NWARPS;
-    // look-back batch (predecessors fetched concurrently): inside a segment the predecessor finished a wave ago, one or two
-    // loads find its inclusive prefix; the plain chained scan over concurrently processed tiles needs a deep batch
-    constexpr int LB = SEG ? TG_LB_SEG : TG_LB;
-    constexpr bool PF = TG_PF != 0;      // request the first batch before the scatter
+    typedef PartCfg<WORDS, DigitFn::kStoreDigit, PEER, DigitFn::kScratch> C;
+    constexpr int THREADS = C::THREADS, ITEMS = C::ITEMS, TILE = C::TILE, NWARPS = C::NWARPS;
+    // look-back batch (predecessors fetched concurrently); the first batch is requested before the scatter.  Inside a segment
+    // the predecessor usually finished a wave ago and one load finds its inclusive prefix, but a dominant segment's tiles
+    // still run concurrently at the tail of the list, and the plain chained scan runs over concurrently processed tiles
+    constexpr int LB = 8;
     static_assert(THREADS >= RADIX, "one thread per digit in the scan phases");
 
     // plain pointer arithmetic on the shared array keeps the shared address space (LDS/STS, 32-bit addresses)
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     Item* const buf0 = reinterpret_cast<Item*>(smem_raw);
-    Item* const buf1 = reinterpret_cast<Item*>(smem_raw + (C::NBUF - 1) * C::BUF_BYTES);
-    cnt_t* const whist = reinterpret_cast<cnt_t*>(smem_raw + C::NBUF * C::BUF_BYTES);  // [NWARPS][RADIX]
+    Item* const buf1 = reinterpret_cast<Item*>(smem_raw + C::BUF_BYTES);
+    cnt_t* const whist = reinterpret_cast<cnt_t*>(smem_raw + 2 * C::BUF_BYTES);  // [NWARPS][RADIX]
     u32* const goff = reinterpret_cast<u32*>(whist + NWARPS * RADIX);            // [RADIX]
     u32* const warp_tot = goff + RADIX;                                          // [16]
     u64* const mbar = reinterpret_cast<u64*>(warp_tot + 16);                     // [2]
@@ -286,11 +262,11 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
     // by ordinary loads.
     auto tma_shift = [&](const TileInfo& ti) -> u32 { return WORDS == 1 ? (ti.start & 1u) : 0u; };
     auto tma_ok = [&](const TileInfo& ti) -> bool {
-        if (!TMA || ti.len != (u32)TILE) return false;
+        if (ti.len != (u32)TILE) return false;
         return tma_shift(ti) == 0 || (size_t)ti.start + TILE + 1 <= n;
     };
 
-    if (TMA && tid == 0) {
+    if (tid == 0) {
         mbar_init(&mbar[0], 1);
         mbar_init(&mbar[1], 1);
         mbar_fence_init();
@@ -301,7 +277,7 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
     u32 j = blockIdx.x;
     TileInfo tnext = tile_info(j < num_tiles ? j : 0);        // descriptors of the tiles of the next two iterations
     TileInfo tnext2 = tile_info(j + gridDim.x < num_tiles ? j + gridDim.x : 0);
-    if (TMA && j < num_tiles) {
+    if (j < num_tiles) {
         const TileInfo t0 = tnext;
         if (tid == 0 && tma_ok(t0)) {
             const u32 sh = tma_shift(t0), bytes = C::TILE_BYTES + 16 * sh;
@@ -312,7 +288,7 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
     u32 phase = 0;        // bit b: parity of the next completion of mbar[b]
 
     for (u32 it = 0; j < num_tiles; j += gridDim.x, ++it) {
-        const int cur = TMA ? (it & 1) : 0;
+        const int cur = it & 1;
         Item* const buf = cur ? buf1 : buf0;
         Item* const nbuf = cur ? buf0 : buf1;
         const TileInfo ti = tnext;
@@ -327,7 +303,7 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
         const u32* const gb = SEG ? sl.segbase + (size_t)ti.seg * RADIX : gbase;
 
         // prefetch the CTA's next tile (TMA unit, async proxy) into the other buffer
-        if (TMA && tid == 0 && j + gridDim.x < num_tiles) {
+        if (tid == 0 && j + gridDim.x < num_tiles) {
             const TileInfo tn = tnext;
             if (tma_ok(tn)) {
                 const u32 sh = tma_shift(tn), bytes = C::TILE_BYTES + 16 * sh;
@@ -368,13 +344,13 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
 
         // ---- stable rank inside the warp (partial tiles always carry the digit along: padding has none)
         if (full_tile && UNSTABLE) rank_rows_unstable<DigitFn::kStoreDigit>(key, rank, fn, whist_w_a, wbase + lane, tile_base);
-        else if (full_tile) rank_rows<true, DigitFn::kStoreDigit>(key, rank, fn, whist_w_a, wbase + lane, tile_base, tile_valid, lt, DBG && (dbg & 2));
+        else if (full_tile) rank_rows<true, DigitFn::kStoreDigit>(key, rank, fn, whist_w_a, wbase + lane, tile_base, tile_valid, lt);
         else rank_rows<false, true>(key, rank, fn, whist_w_a, wbase + lane, tile_base, tile_valid, lt);
         __syncthreads();      // all items are in registers (buf is free), all warp counters final
 
         // ---- per-digit tile count; publish PARTIAL as early as possible; start the look-back loads
         u32 count = 0, my_start = 0;
-        u32 lbv[(PF && !SEG) ? LB : 1];
+        u32 lbv[SEG ? 1 : LB];
         const u32 my_gb = tid < RADIX ? __ldg(&gb[tid]) : 0u;      // (requested early: needed after the look-back)
         u32* const my_status = status + (size_t)ti.row * RADIX + tid;       // predecessor k: my_status - k * RADIX
         if (tid < RADIX) {
@@ -387,10 +363,10 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
                 // inside a segment the predecessor finished a wave of CTAs ago: one load nearly always finds its inclusive prefix
                 lbv[0] = ti.idx > 0 ? ld_relaxed_u32(my_status - RADIX) : FLAG_INCL;
             }
-            else if (PF) {
+            else {
 #pragma unroll
                 for (int k = 0; k < LB; ++k)
-                    lbv[PF ? k : 0] = ((u32)(k + 1) <= ti.idx) ? ld_relaxed_u32(my_status - (size_t)(k + 1) * RADIX) : FLAG_INCL;
+                    lbv[k] = ((u32)(k + 1) <= ti.idx) ? ld_relaxed_u32(my_status - (size_t)(k + 1) * RADIX) : FLAG_INCL;
             }
             u32 incl = count;
 #pragma unroll
@@ -437,7 +413,7 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
         // round trip; the first batch was requested before the scatter)
         if (tid < RADIX) {
             u32 excl = 0;
-            if (ti.idx > 0 && !(DBG && (dbg & 1))) {
+            if (ti.idx > 0) {
                 u32 back = 1;              // distance of the next predecessor to consume
                 bool done = false;
                 u32 v[LB];
@@ -452,14 +428,9 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
                             v[k] = (back + k <= ti.idx) ? ld_relaxed_u32(my_status - (size_t)(back + k) * RADIX) : FLAG_INCL;
                     }
                 }
-                else if (PF) {
-#pragma unroll
-                    for (int k = 0; k < LB; ++k) v[k] = lbv[PF ? k : 0];
-                }
                 else {
 #pragma unroll
-                    for (int k = 0; k < LB; ++k)
-                        v[k] = (back + k <= ti.idx) ? ld_relaxed_u32(my_status - (size_t)(back + k) * RADIX) : FLAG_INCL;
+                    for (int k = 0; k < LB; ++k) v[k] = lbv[k];
                 }
                 while (!done) {
                     bool stalled = false;
@@ -492,10 +463,8 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
                 for (int i = 0; i < ITEMS; ++i) {
                     Item v = bufp[i * THREADS];
                     u32 d = DigitFn::kStoreDigit ? (u32)dig[i * THREADS + tid] : fn(v, 0);
-                    if (DBG && (dbg & 8)) continue;
                     if (DigitFn::kHasDrop && d == RADIX - 1) continue;
-                    if (DBG && (dbg & 4)) out[tile_base + (u32)(i * THREADS + tid)] = v;
-                    else if (PEER) dptr[d][goff[d] + (u32)(i * THREADS + tid)] = v;
+                    if (PEER) dptr[d][goff[d] + (u32)(i * THREADS + tid)] = v;
                     else out[goff[d] + (u32)(i * THREADS + tid)] = v;
                 }
             }
@@ -523,136 +492,53 @@ __global__ void copy_items_kernel(const typename ItemT<WORDS>::type* __restrict_
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = in[i];
 }
 
-// launch configurations (threads per CTA, 8-byte words per thread, CTAs per SM); TG_SWEEP_CFG overrides the default
-struct SweepVariant { int threads, wpt, minb; };
-constexpr SweepVariant kSweepVariants[] = { { 512, 16, 1 }, { 256, 16, 2 }, { 256, 16, 3 }, { 384, 16, 2 },
-                                            { 512, 8, 2 },  { 256, 8, 4 },  { 512, 8, 3 },  { 1024, 8, 1 },
-                                            { 256, 16, 3 }, { 256, 16, 4 }, { 512, 16, 2 } };      // 8..10: no TMA staging
-constexpr int kNumSweepVariants = sizeof(kSweepVariants) / sizeof(kSweepVariants[0]);
-inline int sweep_cfg() {
-    static int cfg = -1;
-    if (cfg < 0) {
-        const char* e = getenv("TG_SWEEP_CFG");
-        // 512 x 16, 1 CTA/SM: measured best on H100 (400 W) for 8- and 16-byte items, Sort 1e8 u64 5.56 ms vs 6.17 ms with
-        // 256 x 16 x 3, ReducePair 1.25e8 Zipf 6.25 ms vs 6.67 ms
-        cfg = e ? atoi(e) : 0;
-        if (cfg < 0 || cfg >= kNumSweepVariants) cfg = 0;
-    }
-    return cfg;
-}
+// items per tile (the host builds tile lists and chunk geometry with it)
 template <int WORDS>
-inline u32 num_tiles_for(size_t n) {
-    const SweepVariant& v = kSweepVariants[sweep_cfg()];
-    u32 tile = (u32)v.threads * (u32)(v.wpt / WORDS);
-    return (u32)((n + tile - 1) / tile);
-}
+constexpr u32 tile_items() { return (u32)PartCfg<WORDS>::TILE; }
+template <int WORDS>
+constexpr u32 num_tiles_for(size_t n) { return (u32)((n + tile_items<WORDS>() - 1) / tile_items<WORDS>()); }
 
-inline int sweep_debug() {
-    static int f = -1;
-    if (f < 0) { const char* e = getenv("TG_SWEEP_DEBUG"); f = e ? atoi(e) : 0; }
-    return f;
-}
-
-template <int WORDS, int THREADS, int WPT, int MINB, class DigitFn, bool SEG = false, bool DBG = false, bool TMA = true, bool PEER = false,
-          bool UNSTABLE = false>
+template <int WORDS, class DigitFn, bool SEG, bool PEER = false, bool UNSTABLE = false>
 int launch_partition_v(tg_ctx* ctx, const void* in, void* out, u32 n, const DigitFn& fn, const u32* gbase, u32* status,
-                       const SegList& sl = SegList{ nullptr, nullptr, 0, nullptr }, typename ItemT<WORDS>::type* const* dbase = nullptr) {
+                       const SegList& sl, typename ItemT<WORDS>::type* const* dbase = nullptr) {
     typedef typename ItemT<WORDS>::type Item;
-    constexpr int IPT = WPT / WORDS;
-    typedef SweepCfg<WORDS, THREADS, IPT, TMA, DigitFn::kStoreDigit, PEER, DigitFn::kScratch> C;
-    auto kern = partition_kernel<WORDS, THREADS, IPT, MINB, DigitFn, SEG, DBG, TMA, PEER, UNSTABLE>;
+    typedef PartCfg<WORDS, DigitFn::kStoreDigit, PEER, DigitFn::kScratch> C;
+    auto kern = partition_kernel<WORDS, DigitFn, SEG, PEER, UNSTABLE>;
     int ctas_per_sm = 0;
     auto it = ctx->kernel_cfg.find((const void*)kern);
     if (it != ctx->kernel_cfg.end()) ctas_per_sm = it->second;
     else {
         TG_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
         // the look-back needs every CTA of the grid resident: size the grid from the real occupancy
-        TG_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, kern, THREADS, C::SMEM));
+        TG_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, kern, C::THREADS, C::SMEM));
         if (ctas_per_sm < 1) return tg_set_error(ctx, TG_ERR_CUDA, "partition kernel does not fit on an SM");
-        if (ctas_per_sm > MINB) ctas_per_sm = MINB;
+        if (ctas_per_sm > C::MIN_BLOCKS) ctas_per_sm = C::MIN_BLOCKS;
         ctx->kernel_cfg[(const void*)kern] = ctas_per_sm;
     }
     u32 num_tiles = SEG ? sl.num_tiles : (n + C::TILE - 1) / C::TILE;
     if (num_tiles == 0) return TG_OK;
     int grid = ctx->sm_count * ctas_per_sm;
     if (grid > (int)num_tiles) grid = (int)num_tiles;
-    TG_LAUNCH_T(ctx, TG_K_PARTITION, kern, grid, THREADS, C::SMEM, (const Item*)in, (Item*)out, n, fn, gbase, status, sl, DBG ? sweep_debug() : 0, dbase);
+    TG_LAUNCH_T(ctx, TG_K_PARTITION, kern, grid, C::THREADS, C::SMEM, (const Item*)in, (Item*)out, n, fn, gbase, status, sl, dbase);
     return TG_OK;
 }
 
 // launch one partition pass with precomputed global bases (status must be zeroed, num_tiles*RADIX words)
 template <int WORDS, class DigitFn>
 int launch_partition(tg_ctx* ctx, const void* in, void* out, u32 n, const DigitFn& fn, const u32* gbase, u32* status) {
-#ifdef TG_DBG_BUILD
-    if (sweep_debug()) {
-        switch (sweep_cfg()) {
-        case 1: return launch_partition_v<WORDS, 256, 16, 2, DigitFn, false, true>(ctx, in, out, n, fn, gbase, status);
-        case 2: return launch_partition_v<WORDS, 256, 16, 3, DigitFn, false, true>(ctx, in, out, n, fn, gbase, status);
-        case 3: return launch_partition_v<WORDS, 384, 16, 2, DigitFn, false, true>(ctx, in, out, n, fn, gbase, status);
-        case 4: return launch_partition_v<WORDS, 512, 8, 2, DigitFn, false, true>(ctx, in, out, n, fn, gbase, status);
-        case 6: return launch_partition_v<WORDS, 512, 8, 3, DigitFn, false, true>(ctx, in, out, n, fn, gbase, status);
-        default: return launch_partition_v<WORDS, 512, 16, 1, DigitFn, false, true>(ctx, in, out, n, fn, gbase, status);
-        }
-    }
-#endif
-    switch (sweep_cfg()) {
-    case 1: return launch_partition_v<WORDS, 256, 16, 2, DigitFn>(ctx, in, out, n, fn, gbase, status);
-    case 2: return launch_partition_v<WORDS, 256, 16, 3, DigitFn>(ctx, in, out, n, fn, gbase, status);
-    case 3: return launch_partition_v<WORDS, 384, 16, 2, DigitFn>(ctx, in, out, n, fn, gbase, status);
-    case 4: return launch_partition_v<WORDS, 512, 8, 2, DigitFn>(ctx, in, out, n, fn, gbase, status);
-    case 5: return launch_partition_v<WORDS, 256, 8, 4, DigitFn>(ctx, in, out, n, fn, gbase, status);
-    case 6: return launch_partition_v<WORDS, 512, 8, 3, DigitFn>(ctx, in, out, n, fn, gbase, status);
-    case 7: return launch_partition_v<WORDS, 1024, 8, 1, DigitFn>(ctx, in, out, n, fn, gbase, status);
-    case 8: return launch_partition_v<WORDS, 256, 16, 3, DigitFn, false, false, false>(ctx, in, out, n, fn, gbase, status);
-    case 9: return launch_partition_v<WORDS, 256, 16, 4, DigitFn, false, false, false>(ctx, in, out, n, fn, gbase, status);
-    case 10: return launch_partition_v<WORDS, 512, 16, 2, DigitFn, false, false, false>(ctx, in, out, n, fn, gbase, status);
-    default: return launch_partition_v<WORDS, 512, 16, 1, DigitFn>(ctx, in, out, n, fn, gbase, status);
-    }
-}
-
-// items per tile of the selected launch configuration (the host builds segmented tile lists with it)
-template <int WORDS>
-inline u32 tile_items() {
-    const SweepVariant& v = kSweepVariants[sweep_cfg()];
-    return (u32)v.threads * (u32)(v.wpt / WORDS);
+    return launch_partition_v<WORDS, DigitFn, false>(ctx, in, out, n, fn, gbase, status, SegList{ nullptr, nullptr, 0, nullptr });
 }
 
 // one partition pass over independent segments (see SegList) of an array of n items; status = sl.num_tiles * RADIX zeroed words
 template <int WORDS, class DigitFn>
 int launch_partition_seg(tg_ctx* ctx, const void* in, void* out, u32 n, const DigitFn& fn, u32* status, const SegList& sl) {
-    switch (sweep_cfg()) {
-    case 1: return launch_partition_v<WORDS, 256, 16, 2, DigitFn, true>(ctx, in, out, n, fn, nullptr, status, sl);
-    case 2: return launch_partition_v<WORDS, 256, 16, 3, DigitFn, true>(ctx, in, out, n, fn, nullptr, status, sl);
-    case 3: return launch_partition_v<WORDS, 384, 16, 2, DigitFn, true>(ctx, in, out, n, fn, nullptr, status, sl);
-    case 4: return launch_partition_v<WORDS, 512, 8, 2, DigitFn, true>(ctx, in, out, n, fn, nullptr, status, sl);
-    case 5: return launch_partition_v<WORDS, 256, 8, 4, DigitFn, true>(ctx, in, out, n, fn, nullptr, status, sl);
-    case 6: return launch_partition_v<WORDS, 512, 8, 3, DigitFn, true>(ctx, in, out, n, fn, nullptr, status, sl);
-    case 7: return launch_partition_v<WORDS, 1024, 8, 1, DigitFn, true>(ctx, in, out, n, fn, nullptr, status, sl);
-    case 8: return launch_partition_v<WORDS, 256, 16, 3, DigitFn, true, false, false>(ctx, in, out, n, fn, nullptr, status, sl);
-    case 9: return launch_partition_v<WORDS, 256, 16, 4, DigitFn, true, false, false>(ctx, in, out, n, fn, nullptr, status, sl);
-    case 10: return launch_partition_v<WORDS, 512, 16, 2, DigitFn, true, false, false>(ctx, in, out, n, fn, nullptr, status, sl);
-    default: return launch_partition_v<WORDS, 512, 16, 1, DigitFn, true>(ctx, in, out, n, fn, nullptr, status, sl);
-    }
+    return launch_partition_v<WORDS, DigitFn, true>(ctx, in, out, n, fn, nullptr, status, sl);
 }
 
-// one segmented pass that need not be stable (see rank_rows_unstable); launch configurations 0-2, the others run the stable pass
-inline int unstable_cfg() {
-    static int cfg = -2;
-    if (cfg == -2) { const char* e = getenv("TG_UNSTABLE_CFG"); cfg = e ? atoi(e) : -1; }
-    return cfg;
-}
+// one segmented pass that need not be stable (see rank_rows_unstable)
 template <int WORDS, class DigitFn>
 int launch_partition_seg_unstable(tg_ctx* ctx, const void* in, void* out, u32 n, const DigitFn& fn, u32* status, const SegList& sl) {
-    // TG_UNSTABLE_CFG = 8 / 9: the unstable passes alone without the TMA double buffer, 3 / 4 CTAs per SM (same 256 x 16 tile)
-    const int cfg = (unstable_cfg() >= 0 && (sweep_cfg() == 2 || sweep_cfg() == 1)) ? unstable_cfg() : sweep_cfg();
-    switch (cfg) {
-    case 0: return launch_partition_v<WORDS, 512, 16, 1, DigitFn, true, false, true, false, true>(ctx, in, out, n, fn, nullptr, status, sl);
-    case 1: return launch_partition_v<WORDS, 256, 16, 2, DigitFn, true, false, true, false, true>(ctx, in, out, n, fn, nullptr, status, sl);
-    case 2: return launch_partition_v<WORDS, 256, 16, 3, DigitFn, true, false, true, false, true>(ctx, in, out, n, fn, nullptr, status, sl);
-    case 8: return launch_partition_v<WORDS, 256, 16, 3, DigitFn, true, false, false, false, true>(ctx, in, out, n, fn, nullptr, status, sl);
-    case 9: return launch_partition_v<WORDS, 256, 16, 4, DigitFn, true, false, false, false, true>(ctx, in, out, n, fn, nullptr, status, sl);
-    default: return launch_partition_seg<WORDS, DigitFn>(ctx, in, out, n, fn, status, sl);
-    }
+    return launch_partition_v<WORDS, DigitFn, true, false, true>(ctx, in, out, n, fn, nullptr, status, sl);
 }
 
 // one segmented partition pass whose buckets are destination workers: bucket d goes to dbase[d] (device array of PEER_MAX
@@ -660,12 +546,7 @@ int launch_partition_seg_unstable(tg_ctx* ctx, const void* in, void* out, u32 n,
 template <int WORDS, class DigitFn>
 int launch_partition_peer(tg_ctx* ctx, const void* in, u32 n, const DigitFn& fn, u32* status, const SegList& sl,
                           typename ItemT<WORDS>::type* const* dbase) {
-    switch (sweep_cfg()) {
-    case 1: return launch_partition_v<WORDS, 256, 16, 2, DigitFn, true, false, true, true>(ctx, in, nullptr, n, fn, nullptr, status, sl, dbase);
-    case 0: return launch_partition_v<WORDS, 512, 16, 1, DigitFn, true, false, true, true>(ctx, in, nullptr, n, fn, nullptr, status, sl, dbase);
-    case 2: return launch_partition_v<WORDS, 256, 16, 3, DigitFn, true, false, true, true>(ctx, in, nullptr, n, fn, nullptr, status, sl, dbase);
-    default: return tg_set_error(ctx, TG_ERR_ARG, "TG_SWEEP_CFG=%d has no peer-store variant (use 0, 1 or 2, or TG_EXCHANGE=nccl)", sweep_cfg());
-    }
+    return launch_partition_v<WORDS, DigitFn, true, true>(ctx, in, nullptr, n, fn, nullptr, status, sl, dbase);
 }
 
 }  // namespace tgp
