@@ -19,7 +19,9 @@
  * tg_classify_scatter, tg_hash_aggregate, tg_hash_partition, tg_sort, tg_reduce_by_key, tg_reduce_to_index and their
  * _file / _dev forms) takes at most 2^30 - 1 items per call and worker (n_local), and a worker receives at most 2^30 - 1
  * items in an exchange: the partition passes count in 30-bit fields.  ReduceToIndex gives each worker fewer than 2^31
- * indices of the result.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
+ * indices of the result.  Merge (tg_merge and its forms) takes at most 2^30 - 1 items in a worker's k inputs together, and gives
+ * each worker at most 2^30 - 1 items of the result; it merges 2..16 inputs of 8- or 16-byte items.  The collective operators
+ * return TG_ERR_TOO_LARGE on every rank or on none.
  ******************************************************************************/
 #ifndef THRILL_GPU_H
 #define THRILL_GPU_H
@@ -271,6 +273,41 @@ int tg_reduce_to_index_dev(tg_ctx* ctx, const tg_kv_desc* desc, const tg_dev_fil
                            const void* neutral_item16, size_t* out_items, uint64_t* out_begin);
 /* bytes this ctx has moved over PCIe through the File codec since tg_init (tests: a GPU -> GPU chain moves none in between) */
 int tg_transfer_bytes(const tg_ctx* ctx, uint64_t* out_h2d, uint64_t* out_d2h);
+
+/* ---- Merge: k globally sorted DIAs into one (DIA::Merge / api::Merge, api/merge.hpp:75-721) --------------------------------
+ * Each input is sorted by the descriptor across the workers (worker w's shard is sorted and precedes worker w+1's).  The result is
+ * the sorted sequence of all N items in the order (key, input index, global position within the input) — one of the outcomes the
+ * reference allows (it leaves equal items of different inputs in unspecified order) — split so that worker d holds the global
+ * ranks [ceil(d*N/p), ceil((d+1)*N/p)).  The reference balances by a randomised multi-sequence selection (MainOp, :465-700); here the
+ * selection is exact: the key of the item at each boundary rank is found one key byte per round on the device (one ncclAllReduce
+ * of 255 counts per boundary per round), then the per-input counts below / equal to it fix the pieces (tg_merge_plan).  The local
+ * merge of the k runs is a tree of stable 2-way merge-path passes (ceil(log2 k) passes; it replaces the multiway merge tree of
+ * PushData, :160-190).  8- or 16-byte items with any key descriptor tg_sort takes for them; desc->stable
+ * is ignored (the result is always deterministic); records, k < 2 and k > 16 are TG_ERR_ARG.  Inputs are read, never modified.
+ * Output of unsorted inputs is unspecified (a permutation of the items), as in the reference. */
+/* on device buffers; *out_dptr as for tg_sort (ctx-owned, valid until the next operator call).  Collective. */
+int tg_merge(tg_ctx* ctx, const tg_key_desc* desc, const void* const* d_inputs, const size_t* n_inputs, uint32_t k,
+             void** out_dptr, size_t* out_n);
+/* the drop-in call (GpuMergeNode::Execute): input j is a device File (dev != NULL) or a host File (its Blocks); the result is
+ * fetched with tg_fetch_output or taken with tg_output_detach.  Device Files are left intact. */
+typedef struct {
+    const tg_dev_file* dev;
+    const tg_block* blocks;
+    size_t nblocks;
+} tg_merge_input;
+int tg_merge_file(tg_ctx* ctx, const tg_key_desc* desc, const tg_merge_input* inputs, uint32_t k, size_t* out_items);
+/* kernel level (parity tests): the selection of the p-worker operator for p simulated workers on one device, with the sum over
+ * the simulated workers' runs in place of the all-reduce.  d_runs[w*k + j] = worker w's shard of input j; writes
+ * out_bounds[(w*k + j)*(p+1) + d] = the first position of run (w, j) that goes to worker d (d = 0..p). */
+int tg_merge_select(tg_ctx* ctx, const tg_key_desc* desc, const void* const* d_runs, const size_t* n_runs, uint32_t p,
+                    uint32_t k, uint64_t* out_bounds);
+/* The split arithmetic of Merge, pure host code (every worker derives the same plan; exported so that the p > 1 logic is
+ * testable without GPUs).  For runs r = w*k + j and d = 0..p, at index r*(p+1) + d: less / equal = items of run r below / equal
+ * to K_d, the key of the item at merged rank targets[d].  bounds = less + clamp(targets[d] - sum(less) - sum(equal of the runs
+ * before (j, w) in input-major order), 0, equal).  TG_ERR_ARG if the counts are inconsistent: targets decreasing, targets[d]
+ * outside [sum(less), sum(less + equal)], or bounds of a run decreasing in d. */
+int tg_merge_plan(uint32_t p, uint32_t k, const uint64_t* targets, const uint64_t* less, const uint64_t* equal,
+                  uint64_t* out_bounds);
 
 /* ---- synthetic inputs of SURVEY.md §8(d), generated on the device (bench / tests support) ------------ */
 int tg_gen_sort_uniform(tg_ctx* ctx, void* d_out, uint64_t begin, uint64_t n, uint64_t seed);

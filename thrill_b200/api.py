@@ -6,6 +6,7 @@ Mirrors (same names, argument meaning and error behaviour) the slice of thrill/a
     DIA<T>::Sort(cmp) / SortStable(cmp)    thrill/api/sort.hpp:800-937
     DIA<T>::ReducePair(reduce_fn)          thrill/api/reduce_by_key.hpp:410-449
     DIA<T>::ReduceByKey(key_ex, reduce_fn) thrill/api/reduce_by_key.hpp:312-363
+    DIA<T>::Merge(second, cmp) / api::Merge thrill/api/merge.hpp:674-721
     DIA<T>::Size / AllGather / Gather      thrill/api/size.hpp, all_gather.hpp, gather.hpp
 A DIA here holds its local shard as a host numpy array — the stand-in for a data::File whose Blocks are
 1 MiB ByteBlocks (data/byte_block.cpp:23-24, data/block_writer.hpp:405-420).  Operators hand the Blocks to the
@@ -140,6 +141,33 @@ def _item_bytes(items):
     return items.dtype.itemsize if items.ndim == 1 else items.shape[1] * items.dtype.itemsize
 
 
+def Merge(compare_function, *dias, **kw):
+    """api::Merge(comparator, dia0, dia1, ...) (api/merge.hpp:674-713): 2..16 DIAs, each sorted by compare_function, of one
+    item type the GPU path recognises (u64 or pair<u64, 8-byte value> ordered by the key; records are not supported)"""
+    if len(dias) < 2:
+        raise capi.ThrillGpuError("Merge: needs at least two DIAs")
+    first = dias[0]
+    for d in dias[1:]:
+        if d.ctx is not first.ctx:
+            raise capi.ThrillGpuError("Merge: the DIAs belong to different contexts")
+        if d.items.dtype != first.items.dtype or d.items.shape[1:] != first.items.shape[1:]:
+            raise capi.ThrillGpuError("Merge: the DIAs hold different item types (%r, %r)" % (first.items.dtype, d.items.dtype))
+    desc, dtype = first._key_desc(compare_function)
+    if desc.item_bytes not in (8, 16):
+        raise capi.ThrillGpuError("Merge: %d-byte records are not supported by the GPU path" % desc.item_bytes)
+    inputs = (capi.MergeInput * len(dias))()
+    keep = []
+    for j, d in enumerate(dias):
+        blocks, nb = d._blocks(d.items)
+        keep.append(blocks)
+        inputs[j].blocks = C.cast(blocks, C.POINTER(capi.Block))
+        inputs[j].nblocks = nb
+    n_out = C.c_size_t()
+    tg = first.ctx.tg
+    tg.ck(tg.L.tg_merge_file(tg.h, C.byref(desc), inputs, len(dias), C.byref(n_out)))
+    return DIA(first.ctx, first._fetch(n_out.value, dtype, desc.item_bytes, kw.get("_pinned_out")))
+
+
 class DIA(object):
     def __init__(self, ctx, items):
         self.ctx = ctx
@@ -191,6 +219,11 @@ class DIA(object):
         tg = self.ctx.tg
         tg.ck(tg.L.tg_sort_file(tg.h, C.byref(desc), blocks, nb, self.ctx._next_seed(), C.byref(n_out)))
         return DIA(self.ctx, self._fetch(n_out.value, dtype, desc.item_bytes, _pinned_out))
+
+    # ---- DIA<T>::Merge (api/merge.hpp:715-721) ---------------------------------------------------------
+    def Merge(self, second_dia, compare_function=None, _pinned_out=None):
+        """merge with another DIA sorted by the same comparator; equal items come out in (input, position) order"""
+        return Merge(compare_function, self, second_dia, _pinned_out=_pinned_out)
 
     def SortStable(self, compare_function=None):
         return self.Sort(compare_function)         # the GPU path is stable by construction

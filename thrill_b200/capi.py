@@ -32,6 +32,11 @@ class DevFile(C.Structure):
     _fields_ = [("dptr", C.c_void_p), ("items", C.c_uint64), ("item_bytes", C.c_uint32), ("reserved", C.c_uint32)]
 
 
+class MergeInput(C.Structure):
+    """tg_merge_input: a device File (dev) or a host File (blocks, nblocks)"""
+    _fields_ = [("dev", C.POINTER(DevFile)), ("blocks", C.POINTER(Block)), ("nblocks", C.c_size_t)]
+
+
 class BlockGeom(C.Structure):
     _fields_ = [("bytes", C.c_uint64), ("first_item", C.c_uint64), ("num_items", C.c_uint64)]
 
@@ -103,6 +108,10 @@ SYMBOLS = [
     ("tg_sort_dev", _i, [_vp, _P(KeyDesc), _P(DevFile), _u64, _P(_sz)]),
     ("tg_reduce_dev", _i, [_vp, _P(KVDesc), _P(DevFile), _P(_sz)]),
     ("tg_reduce_to_index_dev", _i, [_vp, _P(KVDesc), _P(DevFile), _u64, _vp, _P(_sz), _P(_u64)]),
+    ("tg_merge", _i, [_vp, _P(KeyDesc), _P(_vp), _P(_sz), _u32, _P(_vp), _P(_sz)]),
+    ("tg_merge_file", _i, [_vp, _P(KeyDesc), _P(MergeInput), _u32, _P(_sz)]),
+    ("tg_merge_select", _i, [_vp, _P(KeyDesc), _P(_vp), _P(_sz), _u32, _u32, _P(_u64)]),
+    ("tg_merge_plan", _i, [_u32, _u32, _P(_u64), _P(_u64), _P(_u64), _P(_u64)]),
     ("tg_transfer_bytes", _i, [_vp, _P(_u64), _P(_u64)]),
     ("tg_gen_sort_uniform", _i, [_vp, _vp, _u64, _u64, _u64]),
     ("tg_gen_reduce_uniform", _i, [_vp, _vp, _u64, _u64, _u64, _u64, _i]),

@@ -82,5 +82,9 @@ inline int make_key_view(const tg_key_desc* d, KeyView* kv) {
     return TG_OK;
 }
 
+// tg_merge.cu: stable merge of k sorted runs of 8- or 16-byte items into d_out (d_tmp: scratch of the same size), ties to the
+// lower run index
+int merge_runs(tg_ctx* ctx, const KeyView& kv, uint32_t item_bytes, const void* const* runs, const uint64_t* run_items,
+               uint32_t k, void* d_out, void* d_tmp);
 
 }  // namespace tgp

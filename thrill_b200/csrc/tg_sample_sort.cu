@@ -13,8 +13,8 @@
 //     (classification of a sorted, stable shard is a set of p-1 positions: lower_bound by key + the number of equal-key
 //     items with global index <= the splitter's index) -> NCCL Alltoallv of the p contiguous ranges -> k-way merge of the p
 //     received runs.
-// The stand-alone classify+scatter (tg_classify_scatter, the literal TransmitItems) and the k-way merge (tg_kway_merge)
-// are exported for parity tests and ncu captures.
+// The stand-alone classify+scatter (tg_classify_scatter, the literal TransmitItems) is exported for parity tests and ncu
+// captures; the k-way merge (tg_kway_merge) lives in tg_merge.cu.
 #include <algorithm>
 #include <cmath>
 
@@ -236,117 +236,6 @@ __global__ void boundaries_kernel(const typename ItemT<WORDS>::type* __restrict_
     bnd[j] = (u64)lo + tie[j];
 }
 
-// ---- 2-way merge (merge path), stable: ties take from A (the run with the lower index) --------------------
-constexpr int MG_THREADS = 256;
-template <int WORDS> struct MergeCfg { static constexpr int VT = 16 / WORDS; static constexpr int TILE = MG_THREADS * VT; };
-
-template <int WORDS, class Item>
-__device__ __forceinline__ u32 merge_path_search(const Item* A, u32 na, const Item* B, u32 nb, u32 diag, const KeyView& kv) {
-    // number of A items among the first `diag` merged outputs
-    u32 lo = diag > nb ? diag - nb : 0, hi = diag < na ? diag : na;
-    while (lo < hi) {
-        u32 mid = (lo + hi) >> 1;            // take mid+1 items from A?
-        Canon a = canon_key(A[mid], kv);
-        Canon b = canon_key(B[diag - 1 - mid], kv);
-        if (canon_less(b, a)) hi = mid; else lo = mid + 1;      // A[mid] <= B[..] -> A first (stable)
-    }
-    return lo;
-}
-
-template <int WORDS>
-__global__ void __launch_bounds__(MG_THREADS)
-merge2_kernel(const typename ItemT<WORDS>::type* __restrict__ A, u32 na, const typename ItemT<WORDS>::type* __restrict__ B,
-              u32 nb, typename ItemT<WORDS>::type* __restrict__ out, KeyView kv) {
-    typedef typename ItemT<WORDS>::type Item;
-    constexpr int VT = MergeCfg<WORDS>::VT, TILE = MergeCfg<WORDS>::TILE;
-    __shared__ Item sm[TILE + 1];
-    __shared__ u32 split[2];
-    const u32 total = na + nb;
-    const u32 o0 = blockIdx.x * TILE;
-    const u32 o1 = o0 + TILE < total ? o0 + TILE : total;
-    if (threadIdx.x < 2) split[threadIdx.x] = merge_path_search<WORDS>(A, na, B, nb, threadIdx.x ? o1 : o0, kv);
-    __syncthreads();
-    const u32 a0 = split[0], a1 = split[1], b0 = o0 - a0, b1 = o1 - a1;
-    const u32 la = a1 - a0, lb = b1 - b0;
-    for (u32 i = threadIdx.x; i < la; i += MG_THREADS) sm[i] = A[a0 + i];
-    for (u32 i = threadIdx.x; i < lb; i += MG_THREADS) sm[la + i] = B[b0 + i];
-    __syncthreads();
-    const Item* sa = sm;
-    const Item* sb = sm + la;
-    u32 diag = threadIdx.x * VT;
-    if (diag > la + lb) diag = la + lb;
-    u32 ai = merge_path_search<WORDS>(sa, la, sb, lb, diag, kv);
-    u32 bi = diag - ai;
-    Item r[VT];
-#pragma unroll
-    for (int i = 0; i < VT; ++i) {
-        bool take_a;
-        if (ai >= la) take_a = false;
-        else if (bi >= lb) take_a = true;
-        else take_a = !canon_less(canon_key(sb[bi], kv), canon_key(sa[ai], kv));
-        if (ai < la || bi < lb) r[i] = take_a ? sa[ai] : sb[bi];
-        if (take_a) ++ai; else ++bi;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int i = 0; i < VT; ++i)
-        if (threadIdx.x * VT + i < la + lb) sm[threadIdx.x * VT + i] = r[i];
-    __syncthreads();
-    for (u32 i = threadIdx.x; i < la + lb; i += MG_THREADS) out[o0 + i] = sm[i];
-}
-
-template <int WORDS>
-int merge_runs_impl(tg_ctx* ctx, const KeyView& kv, const void* d_runs, const uint64_t* run_items, uint32_t k,
-                    void* d_out, void* d_tmp) {
-    typedef typename ItemT<WORDS>::type Item;
-    constexpr int TILE = MergeCfg<WORDS>::TILE;
-    struct Run { size_t off, len; };
-    std::vector<Run> runs;
-    size_t total = 0;
-    for (uint32_t r = 0; r < k; ++r) { runs.push_back({ total, (size_t)run_items[r] }); total += run_items[r]; }
-    if (total >= (1ull << 31)) return tg_set_error(ctx, TG_ERR_TOO_LARGE, "merge: %zu items", total);
-    // drop empty runs (SortNode has none either: a File is only created for a non-empty vector, :696-704)
-    std::vector<Run> cur;
-    for (auto& r : runs) if (r.len) cur.push_back(r);
-    if (cur.empty()) return TG_OK;
-    int levels = 0;
-    for (size_t c = cur.size(); c > 1; c = (c + 1) / 2) ++levels;
-    // ping-pong so that the last level lands in d_out
-    const Item* src = (const Item*)d_runs;
-    Item* bufs[2] = { (Item*)d_out, (Item*)d_tmp };
-    int which = (levels % 2 == 0) ? 0 : 1;       // buffer written by the first level is bufs[which^...]
-    if (levels == 0) {
-        TG_CUDA(ctx, cudaMemcpyAsync(d_out, src + cur[0].off, cur[0].len * sizeof(Item), cudaMemcpyDeviceToDevice, ctx->stream));
-        return TG_OK;
-    }
-    // level l writes to bufs[(levels - 1 - l) % 2]: the last level (l = levels-1) writes bufs[0] = d_out
-    (void)which;
-    for (int l = 0; l < levels; ++l) {
-        Item* dst = bufs[(levels - 1 - l) % 2];
-        std::vector<Run> next;
-        size_t woff = 0;
-        for (size_t i = 0; i < cur.size(); i += 2) {
-            if (i + 1 < cur.size()) {
-                size_t len = cur[i].len + cur[i + 1].len;
-                u32 grid = (u32)((len + TILE - 1) / TILE);
-                TG_LAUNCH_T(ctx, TG_K_MERGE, merge2_kernel<WORDS>, grid, MG_THREADS, 0, src + cur[i].off, (u32)cur[i].len,
-                          src + cur[i + 1].off, (u32)cur[i + 1].len, dst + woff, kv);
-                next.push_back({ woff, len });
-                woff += len;
-            }
-            else {
-                TG_CUDA(ctx, cudaMemcpyAsync(dst + woff, src + cur[i].off, cur[i].len * sizeof(Item),
-                                             cudaMemcpyDeviceToDevice, ctx->stream));
-                next.push_back({ woff, cur[i].len });
-                woff += cur[i].len;
-            }
-        }
-        cur.swap(next);
-        src = dst;
-    }
-    return TG_OK;
-}
-
 void canon_splitters_from_packed(const tg_key_desc* desc, const KeyView& kv, const void* packed, uint32_t nspl,
                                  std::vector<CanonIdx>* out) {
     const unsigned char* p = (const unsigned char*)packed;
@@ -531,7 +420,9 @@ int sort_multi_impl(tg_ctx* ctx, const tg_key_desc* desc, const KeyView& kv, voi
     TG_TRY(tg_ws_get(ctx, WS_OUT, (n_recv + 1) * s, (void**)&d_out));
     void* d_mtmp;        // (WS_SORT_TMP may still be the send buffer of the exchange)
     TG_TRY(tg_ws_get(ctx, WS_AUX2, (n_recv + 1) * s, &d_mtmp));
-    TG_TRY(merge_runs_impl<WORDS>(ctx, kv, d_recv, (const uint64_t*)recv_cnt.data(), (uint32_t)p, d_out, d_mtmp));
+    const void* runs[TG_MAX_RANKS];
+    for (int r = 0; r < p; ++r) runs[r] = d_recv + recv_off[r];
+    TG_TRY(merge_runs(ctx, kv, (uint32_t)s, runs, (const uint64_t*)recv_cnt.data(), (uint32_t)p, d_out, d_mtmp));
     *out_dptr = d_out;
     *out_n = (size_t)n_recv;
     return TG_OK;
@@ -827,16 +718,6 @@ int tg_classify_scatter(tg_ctx* ctx, const tg_key_desc* desc, const void* d_in, 
     TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     for (uint32_t r = 0; r < p; ++r) out_counts[r] = hc[r];
     return TG_OK;
-}
-
-int tg_kway_merge(tg_ctx* ctx, const tg_key_desc* desc, const void* d_runs, const uint64_t* run_items, uint32_t k,
-                  void* d_out, void* d_tmp) {
-    KeyView kv;
-    if (!ctx || make_key_view(desc, &kv) != TG_OK || (desc->item_bytes != 8 && desc->item_bytes != 16))
-        return tg_set_error(ctx, TG_ERR_ARG, "kway_merge: unsupported descriptor");
-    TG_CUDA(ctx, cudaSetDevice(ctx->device));
-    return desc->item_bytes == 8 ? merge_runs_impl<1>(ctx, kv, d_runs, run_items, k, d_out, d_tmp)
-                                 : merge_runs_impl<2>(ctx, kv, d_runs, run_items, k, d_out, d_tmp);
 }
 
 int tg_sort(tg_ctx* ctx, const tg_key_desc* desc, void* d_in, size_t n_local, uint64_t rng_seed, void** out_dptr, size_t* out_n) {

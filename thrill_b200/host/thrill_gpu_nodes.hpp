@@ -5,6 +5,7 @@
  * (thrill/api/sort.hpp:64-271) and ReduceNode (thrill/api/reduce_by_key.hpp:64-211), and the front doors
  *     thrill_gpu::Sort(dia [, std::less<T>/std::greater<T>])     <->  DIA<T>::Sort      (api/sort.hpp:800)
  *     thrill_gpu::ReducePair(dia, std::plus<double> ...)          <->  DIA<T>::ReducePair(api/reduce_by_key.hpp:410)
+ *     thrill_gpu::Merge(std::less<T>(), dia0, dia1, ...)          <->  api::Merge        (api/merge.hpp:673)
  * Everything else of the pipeline (sources, LOps, other DOps, actions, the net/data layers) is the
  * UNMODIFIED reference library: this header only includes it.  The heavy lifting happens behind the C ABI
  * of include/thrill_gpu.h (libthrill_gpu.so): the nodes hand the Blocks of their input data::File to
@@ -27,6 +28,8 @@
 #include <thrill/api/dop_node.hpp>
 #include <thrill/common/config.hpp>
 #include <thrill/data/file.hpp>
+#include <tlx/meta/call_foreach_with_index.hpp>
+#include <tlx/meta/vexpand.hpp>
 
 #include <array>
 #include <cstdlib>
@@ -239,7 +242,9 @@ class GpuNodeBase
 {
 public:
     virtual ~GpuNodeBase() { }
-    virtual bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes) = 0;
+    //! parent_index: which of the child's parents makes the offer (DIANode::PushFile passes it to OnPreOpFile the same way,
+    //! api/dia_node.hpp:156-177); a parent that feeds two inputs of one child offers once per edge
+    virtual bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes, size_t parent_index) = 0;
 };
 
 //! materialise a device File as a host data::File (the lazy D2H, only for children that are not GPU nodes)
@@ -307,7 +312,7 @@ public:
     }
 
     //! a parent GPU node hands its result over in HBM
-    bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes) final {
+    bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes, size_t /* parent_index */) final {
         if (!parent_stack_empty_ || item_bytes != sizeof(ValueType)) return false;
         device_input_ = file;
         return true;
@@ -343,8 +348,8 @@ public:
     void PushData(bool consume) final {
         if (device_result_ && AllChildrenAreGpuNodes(*this)) {
             bool all = true;
-            for (thrill::api::DIABase* ch : this->children())
-                all = dynamic_cast<GpuNodeBase*>(ch)->OnPreOpDeviceFile(device_result_, sizeof(ValueType)) && all;
+            for (const auto& ch : this->children_)
+                all = dynamic_cast<GpuNodeBase*>(ch.node)->OnPreOpDeviceFile(device_result_, sizeof(ValueType), ch.parent_index) && all;
             if (all) return;
         }
         if (!have_host_file_) {
@@ -402,7 +407,7 @@ public:
         return true;
     }
 
-    bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes) final {
+    bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes, size_t /* parent_index */) final {
         if (!parent_stack_empty_ || item_bytes != sizeof(ValueType)) return false;
         device_input_ = file;
         return true;
@@ -446,8 +451,8 @@ public:
     void PushData(bool consume) final {
         if (device_result_ && AllChildrenAreGpuNodes(*this)) {
             bool all = true;
-            for (thrill::api::DIABase* ch : this->children())
-                all = dynamic_cast<GpuNodeBase*>(ch)->OnPreOpDeviceFile(device_result_, sizeof(ValueType)) && all;
+            for (const auto& ch : this->children_)
+                all = dynamic_cast<GpuNodeBase*>(ch.node)->OnPreOpDeviceFile(device_result_, sizeof(ValueType), ch.parent_index) && all;
             if (all) return;
         }
         if (!have_host_file_) {
@@ -469,6 +474,115 @@ private:
     thrill::data::File::Writer input_writer_;
     thrill::data::File reduced_file_ { context_.GetFile(this) };
     DeviceFilePtr device_input_, device_result_;
+    bool have_host_file_ = false;
+};
+
+//! DIA::Merge / api::Merge (api/merge.hpp:75-721) of kNumInputs DIAs sorted by the same comparator: the MergeNode protocol (one
+//! File per parent, registered with AddChild(this, chain, index), :115-139; OnPreOpFile / StopPreOp per parent) with MainOp and
+//! the multiway merge of PushData behind tg_merge_file.  Any input may arrive as a device File from a parent GPU node.
+template <typename ValueType, size_t kNumInputs>
+class GpuMergeNode final : public thrill::api::DOpNode<ValueType>, public GpuNodeBase
+{
+    using Super = thrill::api::DOpNode<ValueType>;
+    using Super::context_;
+
+public:
+    template <typename ParentDIA0, typename... ParentDIAs>
+    GpuMergeNode(const tg_key_desc& desc, const ParentDIA0& parent0, const ParentDIAs& ... parents)
+        : Super(parent0.ctx(), "GpuMerge", { parent0.id(), parents.id() ... }, { parent0.node(), parents.node() ... }),
+          desc_(desc), parent_stack_empty_({ { ParentDIA0::stack_empty, (ParentDIAs::stack_empty)... } }) {
+        for (size_t i = 0; i < kNumInputs; ++i) {
+            files_[i] = context_.GetFilePtr(this);
+            writers_[i] = files_[i]->GetWriter();
+        }
+        tlx::call_foreach_with_index(RegisterParent(this), parent0, parents ...);
+    }
+
+    //! per-item PreOp of parent Index into its File (api/merge.hpp:115-139)
+    class RegisterParent
+    {
+    public:
+        explicit RegisterParent(GpuMergeNode* node) : node_(node) { }
+        template <typename Index, typename Parent>
+        void operator () (const Index&, Parent& parent) {
+            thrill::data::File::Writer* writer = &node_->writers_[Index::index];
+            auto pre_op_fn = [writer](const ValueType& input) -> void { writer->Put(input); };
+            auto lop_chain = parent.stack().push(pre_op_fn).fold();
+            parent.node()->AddChild(node_, lop_chain, Index::index);
+        }
+
+    private:
+        GpuMergeNode* node_;
+    };
+
+    bool OnPreOpFile(const thrill::data::File& file, size_t parent_index) final {
+        if (!parent_stack_empty_[parent_index]) return false;
+        *files_[parent_index] = file.Copy();
+        return true;
+    }
+
+    bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes, size_t parent_index) final {
+        if (!parent_stack_empty_[parent_index] || item_bytes != sizeof(ValueType)) return false;
+        device_inputs_[parent_index] = file;
+        return true;
+    }
+
+    void StopPreOp(size_t parent_index) final { writers_[parent_index].Close(); }
+
+    DIAMemUse ExecuteMemUse() final { return DIAMemUse::Max(); }
+
+    //! MainOp (:465-700) and the merge of PushData (:160-190) behind tg_merge_file.  Collective.  The result stays in HBM.
+    void Execute() final {
+        tg_ctx* c = WorkerCtx(context_);
+        std::vector<std::unique_ptr<PinnedFileView> > views;
+        std::array<tg_merge_input, kNumInputs> in;
+        for (size_t i = 0; i < kNumInputs; ++i) {
+            if (device_inputs_[i]) {
+                in[i] = tg_merge_input { device_inputs_[i]->get(), nullptr, 0 };
+                continue;
+            }
+            views.emplace_back(new PinnedFileView(*files_[i], context_.local_worker_id()));
+            in[i] = tg_merge_input { nullptr, views.back()->data(), views.back()->size() };
+        }
+        size_t out_items = 0;
+        Check(c, tg_merge_file(c, &desc_, in.data(), static_cast<uint32_t>(kNumInputs), &out_items), "tg_merge_file");
+        views.clear();
+        for (size_t i = 0; i < kNumInputs; ++i) {
+            files_[i]->Clear();
+            device_inputs_[i].reset();
+        }
+        tg_dev_file f;
+        Check(c, tg_output_detach(c, &f), "tg_output_detach");
+        device_result_ = std::make_shared<DeviceFile>(c, f);
+        have_host_file_ = false;
+    }
+
+    DIAMemUse PushDataMemUse() final { return 0; }
+
+    void PushData(bool consume) final {
+        if (device_result_ && AllChildrenAreGpuNodes(*this)) {
+            bool all = true;
+            for (const auto& ch : this->children_)
+                all = dynamic_cast<GpuNodeBase*>(ch.node)->OnPreOpDeviceFile(device_result_, sizeof(ValueType), ch.parent_index) && all;
+            if (all) return;
+        }
+        if (!have_host_file_) {
+            FetchDeviceFileIntoFile(WorkerCtx(context_), context_, *device_result_, sizeof(ValueType), merged_file_);
+            have_host_file_ = true;
+        }
+        this->PushFile(merged_file_, consume);
+    }
+
+    void Dispose() final { merged_file_.Clear(); device_result_.reset(); have_host_file_ = false; }
+
+private:
+    tg_key_desc desc_;
+    const std::array<bool, kNumInputs> parent_stack_empty_;
+    thrill::data::FilePtr files_[kNumInputs];
+    thrill::data::File::Writer writers_[kNumInputs];
+    std::array<DeviceFilePtr, kNumInputs> device_inputs_;
+    thrill::data::File merged_file_ { context_.GetFile(this) };
+    DeviceFilePtr device_result_;
     bool have_host_file_ = false;
 };
 
@@ -536,6 +650,28 @@ auto ReduceToIndex(const DIA<std::pair<Key, Value>, Stack>& dia, const ReduceFun
     using ValueType = std::pair<Key, Value>;
     auto node = tlx::make_counting<GpuReduceNode<ValueType> >(
         dia, tg_kv_desc { 16, ReduceDesc<Value, ReduceFunction>::op }, true, size, neutral_element);
+    return DIA<ValueType>(node);
+}
+
+template <bool...> struct BoolPack { };
+template <bool... B> using AllOf = std::is_same<BoolPack<true, B...>, BoolPack<B..., true> >;
+
+//! api::Merge(comparator, dia0, dia1, ...) (api/merge.hpp:673-713) of 2..16 DIAs for the (type, comparator) pairs thrill_gpu::Sort
+//! recognises with 8- or 16-byte items.  Equal items come out in (input, position) order, one of the orders the stock
+//! operator allows.  DIA::Merge(second, cmp) (:715-721) is Merge(cmp, dia, second).
+template <typename Comparator, typename FirstDIA, typename... DIAs>
+auto Merge(const Comparator& /* comparator */, const FirstDIA& first_dia, const DIAs& ... dias) {
+    using ValueType = typename FirstDIA::ValueType;
+    static_assert(SortDesc<ValueType, Comparator>::supported && (sizeof(ValueType) == 8 || sizeof(ValueType) == 16),
+                  "thrill_gpu::Merge: this (ValueType, Comparator) pair has no GPU descriptor for Merge (8- or 16-byte items); "
+                  "use the stock api::Merge(cmp, dias...)");
+    static_assert(sizeof ... (DIAs) >= 1 && sizeof ... (DIAs) <= 15, "thrill_gpu::Merge: 2..16 DIAs");
+    static_assert(AllOf<std::is_same<typename DIAs::ValueType, ValueType>::value ...>::value,
+                  "thrill_gpu::Merge: every DIA must have the same item type");
+    first_dia.AssertValid();
+    tlx::vexpand((dias.AssertValid(), 0) ...);
+    auto node = tlx::make_counting<GpuMergeNode<ValueType, 1 + sizeof ... (DIAs)> >(
+        SortDesc<ValueType, Comparator>::make(), first_dia, dias ...);
     return DIA<ValueType>(node);
 }
 
