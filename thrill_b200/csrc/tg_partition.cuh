@@ -3,13 +3,14 @@
 //   * the splitter classify/scatter (digit = destination worker by the splitters)   tg_sample_sort.cu
 //   * the hash aggregation          (digit = a byte of Hash128to64(0,key), or % p)  tg_reduce.cu
 //
-// Persistent CTAs walk a list of tiles in static round-robin order.  A tile (64 KB) is staged into shared memory by
-// the TMA unit (cp.async.bulk + mbarrier, double buffered: the next tile lands while the current one is processed), ranked
-// stably with warp-synchronous ballots + warp-private counters, positioned by a chained scan with batched decoupled
-// look-back over the tiles of its SEGMENT (the whole input for the plain pass; see tg_segmented.cuh for the chunked and
-// segmented passes whose tile lists never make a tile wait for a concurrently processed one), reordered by digit inside the
-// (re-used) landing buffer and written out so that consecutive threads write consecutive addresses.
-// HBM traffic: read n*s + write n*s + ~3 % scan state.
+// Persistent CTAs walk a list of tiles in static round-robin order.  A tile (128 KB) is staged into shared memory by
+// the TMA unit (cp.async.bulk + mbarrier; the next tile's copy starts as soon as the current tile is in registers and lands
+// while it is processed), ranked stably with warp-synchronous ballots + warp-private counters, positioned by a chained scan
+// with batched decoupled look-back over the tiles of its SEGMENT (the whole input for the plain pass; see tg_segmented.cuh for
+// the chunked and segmented passes whose tile lists never make a tile wait for a concurrently processed one), reordered by
+// digit through a half-tile exchange buffer in two rounds and written out so that consecutive threads write consecutive
+// addresses.
+// HBM traffic: read n*s + write n*s + ~1.5 % scan state.
 #pragma once
 #include "tg_common.cuh"
 
@@ -87,23 +88,28 @@ __device__ __forceinline__ u32 match_digit8(u32 d) {
     return peers;
 }
 
-// Launch configuration of the partition pass: 512 threads per CTA, each owning 16 8-byte words (16 u64 items or 8 16-byte
-// items), one CTA per SM.  On H100 this was the fastest of the configurations measured for 8- and 16-byte items (see
-// DESIGN.md §5).  Tile sizes: 8192 items of 8 bytes, 4096 of 16 bytes.
+// Launch configuration of the partition pass: 512 threads per CTA, each owning 32 8-byte words (32 u64 items or 16 16-byte
+// items), one CTA per SM: tiles of 16384 items of 8 bytes, 8192 of 16 bytes (128 KB).  The tile size is what sets the pass's
+// DRAM efficiency: a tile's write-out is one run per digit, 256 runs of TILE/256 items on average at arbitrary offsets, and
+// the longer the runs the fewer partial 32-byte sectors the writes leave (DESIGN.md §5 has the measured per-tile-size times).
+// A 128 KB tile cannot be double buffered, so the landing buffer is single (the next tile's copy is started as soon as the
+// current tile's items are in registers) and the exchange buffer holds half a tile: the write-out runs in two rounds.
 constexpr int PEER_MAX = 32;        // destinations of a partition pass that stores into peer windows (<= TG_MAX_RANKS used)
 template <int WORDS, bool STORE = true, bool PEER = false, int SCRATCH = 0>
 struct PartCfg {
     static constexpr int THREADS = 512;
     static constexpr int MIN_BLOCKS = 1;                     // CTAs per SM
     static constexpr int ITEM_BYTES = 8 * WORDS;
-    static constexpr int ITEMS = 16 / WORDS;                 // items per thread
-    static constexpr int TILE = THREADS * ITEMS;             // items per tile
+    static constexpr int ITEMS = 32 / WORDS;                 // items per thread
+    static constexpr int TILE = THREADS * ITEMS;             // items per tile (< 65536: 16-bit warp counters and ranks)
+    static constexpr int HALF = TILE / 2;                    // items per exchange round
     static constexpr int TILE_BYTES = TILE * ITEM_BYTES;
     static constexpr int NWARPS = THREADS / 32;
     static constexpr int BUF_BYTES = TILE_BYTES + (WORDS == 1 ? 16 : 0);      // + one 16-byte granule: tiles that start at an odd 8-byte item
-    // 2 landing/exchange buffers | warp counters [NWARPS][RADIX] | goff [RADIX] | warp_tot [16] | mbar [2] | digit bytes [TILE]
-    // (only if the digit function's result is kept, kStoreDigit) | peer pointers [PEER_MAX] | functor scratch | slack
-    static constexpr int SMEM = 2 * BUF_BYTES + NWARPS * RADIX * (int)sizeof(unsigned short) + RADIX * 4 + 64 + 16 + (STORE ? TILE : 0) + (PEER ? PEER_MAX * 8 : 0) + SCRATCH + 128;
+    // landing buffer | exchange buffer [HALF] | warp counters [NWARPS][RADIX] | goff [RADIX] | warp_tot [16] | mbar | digit
+    // bytes [HALF] (only if the digit function's result is kept, kStoreDigit) | peer pointers [PEER_MAX] | functor scratch | slack
+    static constexpr int SMEM = BUF_BYTES + HALF * ITEM_BYTES + NWARPS * RADIX * (int)sizeof(unsigned short) + RADIX * 4 + 64 + 16 + (STORE ? HALF : 0) + (PEER ? PEER_MAX * 8 : 0) + SCRATCH + 128;
+    static_assert(SMEM <= 227 * 1024, "partition pass: shared memory of one CTA");
 };
 
 // exclusive scan of npass digit histograms -> global bases; skip[p] = 1 if one bin holds everything
@@ -201,8 +207,9 @@ struct SegList {
 };
 __device__ __forceinline__ u32 seg_num_tiles(const SegList& sl) { return sl.num_tiles_dev ? __ldg(sl.num_tiles_dev) : sl.num_tiles; }
 
-// One tile: rank -> per-digit counts (published for the chained scan) -> scatter into the exchange buffer while
-// the look-back loads are in flight -> resolve the look-back -> coalesced write-out.
+// One tile: rank -> start the next tile's copy -> per-digit counts (published for the chained scan) -> scatter the first
+// half of the tile's positions into the exchange buffer while the look-back loads are in flight -> resolve the look-back ->
+// coalesced write-out -> scatter and write out the second half.
 // PEER: the buckets are destination workers; bucket d is written to dbase[d][position], where dbase[d] points into worker
 // d's exchange window (mapped peer memory: the stores travel over NVLink) biased so that `position` is the position the
 // plain pass would have used in `out` — the Alltoallv of the reference's MixStream exchange happens inside the pass.
@@ -213,7 +220,7 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
                  typename ItemT<WORDS>::type* const* __restrict__ dbase) {
     typedef typename ItemT<WORDS>::type Item;
     typedef PartCfg<WORDS, DigitFn::kStoreDigit, PEER, DigitFn::kScratch> C;
-    constexpr int THREADS = C::THREADS, ITEMS = C::ITEMS, TILE = C::TILE, NWARPS = C::NWARPS;
+    constexpr int THREADS = C::THREADS, ITEMS = C::ITEMS, TILE = C::TILE, HALF = C::HALF, NWARPS = C::NWARPS;
     // look-back batch (predecessors fetched concurrently); the first batch is requested before the scatter.  Inside a segment
     // the predecessor usually finished a wave ago and one load finds its inclusive prefix, but a dominant segment's tiles
     // still run concurrently at the tail of the list, and the plain chained scan runs over concurrently processed tiles
@@ -222,14 +229,14 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
 
     // plain pointer arithmetic on the shared array keeps the shared address space (LDS/STS, 32-bit addresses)
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    Item* const buf0 = reinterpret_cast<Item*>(smem_raw);
-    Item* const buf1 = reinterpret_cast<Item*>(smem_raw + C::BUF_BYTES);
-    cnt_t* const whist = reinterpret_cast<cnt_t*>(smem_raw + 2 * C::BUF_BYTES);  // [NWARPS][RADIX]
+    Item* const buf = reinterpret_cast<Item*>(smem_raw);                         // landing buffer
+    Item* const xbuf = reinterpret_cast<Item*>(smem_raw + C::BUF_BYTES);         // exchange buffer [HALF]
+    cnt_t* const whist = reinterpret_cast<cnt_t*>(xbuf + HALF);                  // [NWARPS][RADIX]
     u32* const goff = reinterpret_cast<u32*>(whist + NWARPS * RADIX);            // [RADIX]
     u32* const warp_tot = goff + RADIX;                                          // [16]
-    u64* const mbar = reinterpret_cast<u64*>(warp_tot + 16);                     // [2]
-    unsigned char* const dig = reinterpret_cast<unsigned char*>(mbar + 2);       // [TILE], only if kStoreDigit
-    Item** const dptr = reinterpret_cast<Item**>(dig + (DigitFn::kStoreDigit ? TILE : 0));      // [PEER_MAX], only if PEER
+    u64* const mbar = reinterpret_cast<u64*>(warp_tot + 16);                     // the landing buffer's (16 bytes reserved)
+    unsigned char* const dig = reinterpret_cast<unsigned char*>(mbar + 2);       // [HALF], only if kStoreDigit
+    Item** const dptr = reinterpret_cast<Item**>(dig + (DigitFn::kStoreDigit ? HALF : 0));      // [PEER_MAX], only if PEER
     unsigned char* const fscratch = reinterpret_cast<unsigned char*>(dptr + (PEER ? PEER_MAX : 0));  // [kScratch], the functor's
 
     DigitFn fn = fn_param;
@@ -268,7 +275,6 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
 
     if (tid == 0) {
         mbar_init(&mbar[0], 1);
-        mbar_init(&mbar[1], 1);
         mbar_fence_init();
     }
     if (PEER && tid < PEER_MAX) dptr[tid] = dbase[tid];
@@ -282,17 +288,14 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
         if (tid == 0 && tma_ok(t0)) {
             const u32 sh = tma_shift(t0), bytes = C::TILE_BYTES + 16 * sh;
             mbar_expect_tx(&mbar[0], bytes);
-            bulk_g2s(buf0, in + (t0.start - sh), bytes, &mbar[0]);
+            bulk_g2s(buf, in + (t0.start - sh), bytes, &mbar[0]);
         }
     }
-    u32 phase = 0;        // bit b: parity of the next completion of mbar[b]
+    u32 phase = 0;        // parity of the next completion of mbar[0]
 
-    for (u32 it = 0; j < num_tiles; j += gridDim.x, ++it) {
-        const int cur = it & 1;
-        Item* const buf = cur ? buf1 : buf0;
-        Item* const nbuf = cur ? buf0 : buf1;
+    for (; j < num_tiles; j += gridDim.x) {
         const TileInfo ti = tnext;
-        // (descriptors are fetched two tiles ahead: the one of the next tile, needed right below to start its TMA copy, was
+        // (descriptors are fetched two tiles ahead: the one of the next tile, needed below to start its TMA copy, was
         // requested a whole tile ago)
         if (j + gridDim.x < num_tiles) tnext = tnext2;
         if (SEG ? (j + 2 * gridDim.x < num_tiles) : true) tnext2 = tile_info(j + 2 * gridDim.x);
@@ -302,28 +305,18 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
         const bool by_tma = tma_ok(ti);
         const u32* const gb = SEG ? sl.segbase + (size_t)ti.seg * RADIX : gbase;
 
-        // prefetch the CTA's next tile (TMA unit, async proxy) into the other buffer
-        if (tid == 0 && j + gridDim.x < num_tiles) {
-            const TileInfo tn = tnext;
-            if (tma_ok(tn)) {
-                const u32 sh = tma_shift(tn), bytes = C::TILE_BYTES + 16 * sh;
-                fence_proxy_async();
-                mbar_expect_tx(&mbar[cur ^ 1], bytes);
-                bulk_g2s(nbuf, in + (tn.start - sh), bytes, &mbar[cur ^ 1]);
-            }
-        }
         // zero this warp's private digit counters
 #pragma unroll
         for (int i = 0; i < RADIX / 64; ++i) reinterpret_cast<u32*>(whist_w)[i * 32 + lane] = 0;
 
         // ---- items to registers: warp w owns tile positions [w*32*ITEMS, (w+1)*32*ITEMS), round-striped.
         // Positions past the end of a partial tile get digit RADIX-1: the stable ranking puts them behind every
-        // valid item, so they fall off the end of the exchange buffer and are never written.
+        // valid item, so they land past tile_valid and are never written.
         Item key[ITEMS];
         u32 rank[ITEMS];                 // rank inside the (warp, digit) group | digit << 16 (if kStoreDigit)
         if (by_tma) {
-            mbar_wait(&mbar[cur], (phase >> cur) & 1u);
-            phase ^= 1u << cur;
+            mbar_wait(&mbar[0], phase);
+            phase ^= 1u;
             const Item* src = buf + tma_shift(ti) + wbase + lane;
 #pragma unroll
             for (int i = 0; i < ITEMS; ++i) key[i] = src[i * 32];
@@ -347,6 +340,17 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
         else if (full_tile) rank_rows<true, DigitFn::kStoreDigit>(key, rank, fn, whist_w_a, wbase + lane, tile_base, tile_valid, lt);
         else rank_rows<false, true>(key, rank, fn, whist_w_a, wbase + lane, tile_base, tile_valid, lt);
         __syncthreads();      // all items are in registers (buf is free), all warp counters final
+
+        // start the CTA's next tile (TMA unit, async proxy) into the landing buffer: it has the rest of this tile's time to land
+        if (tid == 0 && j + gridDim.x < num_tiles) {
+            const TileInfo tn = tnext;
+            if (tma_ok(tn)) {
+                const u32 sh = tma_shift(tn), bytes = C::TILE_BYTES + 16 * sh;
+                fence_proxy_async();
+                mbar_expect_tx(&mbar[0], bytes);
+                bulk_g2s(buf, in + (tn.start - sh), bytes, &mbar[0]);
+            }
+        }
 
         // ---- per-digit tile count; publish PARTIAL as early as possible; start the look-back loads
         u32 count = 0, my_start = 0;
@@ -391,97 +395,106 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
         }
         __syncthreads();
 
-        // ---- scatter registers -> digit-ordered exchange buffer (reuses the landing buffer)
-        if (full_tile && !DigitFn::kStoreDigit) {
+        // ---- two exchange rounds by tile-local position q: round r moves the items with q in [r*HALF, (r+1)*HALF) through the
+        // exchange buffer (any digit skew takes exactly two rounds; a digit run may straddle them)
 #pragma unroll
-            for (int i = 0; i < ITEMS; ++i) {
-                u32 d = fn(key[i], 0);
-                buf[lds_cnt(whist_w_a + d * (u32)sizeof(cnt_t)) + rank[i]] = key[i];
-            }
-        }
-        else {
-#pragma unroll
-            for (int i = 0; i < ITEMS; ++i) {
-                u32 d = rank[i] >> 16;
-                u32 q = lds_cnt(whist_w_a + d * (u32)sizeof(cnt_t)) + (rank[i] & 0xffffu);
-                buf[q] = key[i];
-                if (DigitFn::kStoreDigit) dig[q] = (unsigned char)d;
-            }
-        }
-
-        // ---- decoupled look-back inside the tile's segment (threads 0..RADIX-1, one digit each, LB predecessors per
-        // round trip; the first batch was requested before the scatter)
-        if (tid < RADIX) {
-            u32 excl = 0;
-            if (ti.idx > 0) {
-                u32 back = 1;              // distance of the next predecessor to consume
-                bool done = false;
-                u32 v[LB];
-                if (SEG) {
-                    // fast path: the prefetched predecessor carries an inclusive prefix.  Otherwise (tiles of a dominant segment that
-                    // run at the same time) continue with batches of LB predecessors per round trip.
-                    if (lbv[0] & FLAG_INCL) { excl = lbv[0] & VALUE_MASK; done = true; }
-                    else {
-                        v[0] = lbv[0];
-#pragma unroll
-                        for (int k = 1; k < LB; ++k)
-                            v[k] = (back + k <= ti.idx) ? ld_relaxed_u32(my_status - (size_t)(back + k) * RADIX) : FLAG_INCL;
-                    }
-                }
-                else {
-#pragma unroll
-                    for (int k = 0; k < LB; ++k) v[k] = lbv[k];
-                }
-                while (!done) {
-                    bool stalled = false;
-#pragma unroll
-                    for (int k = 0; k < LB; ++k) {
-                        if (!done && !stalled) {
-                            if (v[k] & FLAG_INCL) { excl += v[k] & VALUE_MASK; done = true; }
-                            else if (v[k] & FLAG_PARTIAL) { excl += v[k] & VALUE_MASK; back++; }
-                            else stalled = true;
-                        }
-                    }
-                    if (done) break;
-#pragma unroll
-                    for (int k = 0; k < LB; ++k)
-                        v[k] = (back + k <= ti.idx) ? ld_relaxed_u32(my_status - (size_t)(back + k) * RADIX) : FLAG_INCL;
-                }
-                u32 pub = count;
-                if (!full_tile && tid == RADIX - 1) pub -= (u32)TILE - tile_valid;
-                st_relaxed_u32(my_status, (excl + pub) | FLAG_INCL);
-            }
-            goff[tid] = my_gb + excl - my_start;
-        }
-        __syncthreads();
-
-        // ---- coalesced write-out: consecutive threads write consecutive addresses inside a digit run
-        {
-            const Item* const bufp = buf + tid;
-            if (full_tile) {
+        for (int r = 0; r < 2; ++r) {
+            // ---- scatter registers -> digit-ordered exchange buffer
+            if (full_tile && !DigitFn::kStoreDigit) {
 #pragma unroll
                 for (int i = 0; i < ITEMS; ++i) {
-                    Item v = bufp[i * THREADS];
-                    u32 d = DigitFn::kStoreDigit ? (u32)dig[i * THREADS + tid] : fn(v, 0);
-                    if (DigitFn::kHasDrop && d == RADIX - 1) continue;
-                    if (PEER) dptr[d][goff[d] + (u32)(i * THREADS + tid)] = v;
-                    else out[goff[d] + (u32)(i * THREADS + tid)] = v;
+                    u32 d = fn(key[i], 0);
+                    u32 q = lds_cnt(whist_w_a + d * (u32)sizeof(cnt_t)) + rank[i] - (u32)(r * HALF);
+                    if (q < (u32)HALF) xbuf[q] = key[i];
                 }
             }
             else {
 #pragma unroll
                 for (int i = 0; i < ITEMS; ++i) {
-                    if ((u32)(i * THREADS + tid) < tile_valid) {
-                        Item v = bufp[i * THREADS];
-                        u32 d = DigitFn::kStoreDigit ? (u32)dig[i * THREADS + tid] : fn(v, 0);
-                        if (DigitFn::kHasDrop && d == RADIX - 1) continue;
-                        if (PEER) dptr[d][goff[d] + (u32)(i * THREADS + tid)] = v;
-                        else out[goff[d] + (u32)(i * THREADS + tid)] = v;
+                    u32 d = rank[i] >> 16;
+                    u32 q = lds_cnt(whist_w_a + d * (u32)sizeof(cnt_t)) + (rank[i] & 0xffffu) - (u32)(r * HALF);
+                    if (q < (u32)HALF) {
+                        xbuf[q] = key[i];
+                        if (DigitFn::kStoreDigit) dig[q] = (unsigned char)d;
                     }
                 }
             }
+
+            // ---- decoupled look-back inside the tile's segment (threads 0..RADIX-1, one digit each, LB predecessors per
+            // round trip; the first batch was requested before the first scatter)
+            if (r == 0 && tid < RADIX) {
+                u32 excl = 0;
+                if (ti.idx > 0) {
+                    u32 back = 1;              // distance of the next predecessor to consume
+                    bool done = false;
+                    u32 v[LB];
+                    if (SEG) {
+                        // fast path: the prefetched predecessor carries an inclusive prefix.  Otherwise (tiles of a dominant segment that
+                        // run at the same time) continue with batches of LB predecessors per round trip.
+                        if (lbv[0] & FLAG_INCL) { excl = lbv[0] & VALUE_MASK; done = true; }
+                        else {
+                            v[0] = lbv[0];
+#pragma unroll
+                            for (int k = 1; k < LB; ++k)
+                                v[k] = (back + k <= ti.idx) ? ld_relaxed_u32(my_status - (size_t)(back + k) * RADIX) : FLAG_INCL;
+                        }
+                    }
+                    else {
+#pragma unroll
+                        for (int k = 0; k < LB; ++k) v[k] = lbv[k];
+                    }
+                    while (!done) {
+                        bool stalled = false;
+#pragma unroll
+                        for (int k = 0; k < LB; ++k) {
+                            if (!done && !stalled) {
+                                if (v[k] & FLAG_INCL) { excl += v[k] & VALUE_MASK; done = true; }
+                                else if (v[k] & FLAG_PARTIAL) { excl += v[k] & VALUE_MASK; back++; }
+                                else stalled = true;
+                            }
+                        }
+                        if (done) break;
+#pragma unroll
+                        for (int k = 0; k < LB; ++k)
+                            v[k] = (back + k <= ti.idx) ? ld_relaxed_u32(my_status - (size_t)(back + k) * RADIX) : FLAG_INCL;
+                    }
+                    u32 pub = count;
+                    if (!full_tile && tid == RADIX - 1) pub -= (u32)TILE - tile_valid;
+                    st_relaxed_u32(my_status, (excl + pub) | FLAG_INCL);
+                }
+                goff[tid] = my_gb + excl - my_start;
+            }
+            __syncthreads();
+
+            // ---- coalesced write-out: consecutive threads write consecutive addresses inside a digit run
+            {
+                const Item* const bufp = xbuf + tid;
+                const u32 q0 = (u32)(r * HALF) + tid;        // tile-local position of bufp[0]
+                if (full_tile) {
+#pragma unroll
+                    for (int i = 0; i < HALF / THREADS; ++i) {
+                        Item v = bufp[i * THREADS];
+                        u32 d = DigitFn::kStoreDigit ? (u32)dig[i * THREADS + tid] : fn(v, 0);
+                        if (DigitFn::kHasDrop && d == RADIX - 1) continue;
+                        if (PEER) dptr[d][goff[d] + q0 + (u32)(i * THREADS)] = v;
+                        else out[goff[d] + q0 + (u32)(i * THREADS)] = v;
+                    }
+                }
+                else {
+#pragma unroll
+                    for (int i = 0; i < HALF / THREADS; ++i) {
+                        if (q0 + (u32)(i * THREADS) < tile_valid) {
+                            Item v = bufp[i * THREADS];
+                            u32 d = DigitFn::kStoreDigit ? (u32)dig[i * THREADS + tid] : fn(v, 0);
+                            if (DigitFn::kHasDrop && d == RADIX - 1) continue;
+                            if (PEER) dptr[d][goff[d] + q0 + (u32)(i * THREADS)] = v;
+                            else out[goff[d] + q0 + (u32)(i * THREADS)] = v;
+                        }
+                    }
+                }
+            }
+            __syncthreads();      // the exchange buffer is free for the next round or tile
         }
-        __syncthreads();      // exchange buffer is re-armed as the TMA landing buffer two iterations later
     }
 }
 
