@@ -34,3 +34,10 @@ for k, nm in enumerate(names):
     t, cnt = c.profile_get(k)
     if cnt: parts.append("%s %.3f ms/%d" % (nm, t / cnt, cnt))
 print("reduce %s %s n=%d best %.3f ms = %.2f Grec/s distinct=%d | %s" % (op, "uniform" if uniform else "zipf", n, best, n / best / 1e6, rc.value, " | ".join(parts)), flush=True)
+# per-launch partition times in launch order (fastest of the profiled calls at each position)
+profiled = iters - iters // 2
+per = c.profile_list(capi.K_PARTITION)
+k = len(per) // profiled if profiled else 0
+if k:
+    lst = [min(per[s * k + i] for s in range(profiled)) for i in range(k)]
+    print("partition per launch: " + " ".join("%.4f" % t for t in lst) + " ms", flush=True)

@@ -25,3 +25,10 @@ ok = c.is_sorted(desc, d, n) and c.checksum(d, n, 8) == cs0
 print("n=%d best %.3f ms = %.2f Gkeys/s | partition %.4f ms/launch (%d) = %.0f GB/s | hist %.4f ms | fixup %.4f ms (%d) | segcount %.4f ms (%d) | correct=%s"
       % (n, best, n / best / 1e6, pm / max(pc, 1), pc,
          16 * n / (pm / max(pc, 1)) / 1e6, hm / max(hc, 1), fm / max(fc, 1), fc, sm / max(sc, 1), sc, ok), flush=True)
+# per-launch partition times in launch order (fastest of the profiled sorts at each position)
+profiled = iters - iters // 2
+per = c.profile_list(capi.K_PARTITION)
+k = len(per) // profiled if profiled else 0
+if k:
+    lst = [min(per[s * k + i] for s in range(profiled)) for i in range(k)]
+    print("partition per launch: " + " ".join("%.4f" % t for t in lst) + " ms", flush=True)

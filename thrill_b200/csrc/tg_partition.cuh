@@ -7,7 +7,7 @@
 // the TMA unit (cp.async.bulk + mbarrier; the next tile's copy starts as soon as the current tile is in registers and lands
 // while it is processed), ranked stably with warp-synchronous ballots + warp-private counters, positioned by a chained scan
 // with batched decoupled look-back over the tiles of its SEGMENT (the whole input for the plain pass; see tg_segmented.cuh for
-// the chunked and segmented passes whose tile lists never make a tile wait for a concurrently processed one), reordered by
+// the chunked and segmented passes whose tile lists make a tile wait at most for the few tiles of its group), reordered by
 // digit through a half-tile exchange buffer in two rounds and written out so that consecutive threads write consecutive
 // addresses.
 // HBM traffic: read n*s + write n*s + ~1.5 % scan state.
@@ -111,6 +111,11 @@ struct PartCfg {
     static constexpr int SMEM = BUF_BYTES + HALF * ITEM_BYTES + NWARPS * RADIX * (int)sizeof(unsigned short) + RADIX * 4 + 64 + 16 + (STORE ? HALF : 0) + (PEER ? PEER_MAX * 8 : 0) + SCRATCH + 128;
     static_assert(SMEM <= 227 * 1024, "partition pass: shared memory of one CTA");
 };
+// Tiles of one segment that the tile list of a segmented pass (tg_segmented.cuh) puts next to each other.  Neighbouring tiles
+// of a segment write neighbouring runs of every digit, so a group that runs in one wave writes each digit as one run G tiles
+// long instead of G isolated ones (DESIGN.md §5 has the measured per-group-size times).  A group member finds the counts of
+// the members before it with the first batch of its look-back (G <= LB in partition_kernel).
+constexpr u32 TILE_GROUP = 8;
 
 // exclusive scan of npass digit histograms -> global bases; skip[p] = 1 if one bin holds everything
 static __global__ void scan_hist_kernel(const u32* __restrict__ ghist, u32* __restrict__ gbase, u32* __restrict__ skip,
@@ -194,9 +199,10 @@ __device__ __forceinline__ void rank_rows_unstable(const Item (&key)[ITEMS], u32
 
 // Segmented operation: the input is a sequence of independent segments (e.g. the 256 buckets of a previous pass on
 // a more significant digit); every segment is partitioned on its own, with its own bases and its own chained scan.
-// The host lists the tiles in an order that interleaves the segments, so the tile a tile's scan depends on (the
-// previous tile of the same segment) was processed a whole wave of CTAs earlier: the look-back finds its inclusive
-// prefix with one load instead of waiting for tiles that are being processed at the same time.
+// The tile list interleaves groups of TILE_GROUP neighbouring tiles of the segments, so the tile the scan of a group's
+// first tile depends on (the previous tile of the same segment) was processed a whole wave of CTAs earlier: the look-back
+// finds its inclusive prefix with one load.  The other members of a group run at the same time as the members before
+// them, which publish their counts right after ranking; one batch of the look-back reaches back past the group.
 //   tiles[j] = { first item, items (<= TILE), status row, (segment << 20) | index of the tile inside its segment }
 //   status rows of one segment are consecutive; segbase[segment][RADIX] = output position of the segment's digit d.
 struct SegList {
@@ -222,9 +228,11 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
     typedef PartCfg<WORDS, DigitFn::kStoreDigit, PEER, DigitFn::kScratch> C;
     constexpr int THREADS = C::THREADS, ITEMS = C::ITEMS, TILE = C::TILE, HALF = C::HALF, NWARPS = C::NWARPS;
     // look-back batch (predecessors fetched concurrently); the first batch is requested before the scatter.  Inside a segment
-    // the predecessor usually finished a wave ago and one load finds its inclusive prefix, but a dominant segment's tiles
-    // still run concurrently at the tail of the list, and the plain chained scan runs over concurrently processed tiles
+    // the predecessor of a group's first tile usually finished a wave ago and one load finds its inclusive prefix; the other
+    // members of a group, a dominant segment's tiles at the tail of the list and the plain chained scan run concurrently with
+    // their predecessors
     constexpr int LB = 8;
+    static_assert(TILE_GROUP <= (u32)LB, "a group member reaches past its group's first tile with one batch");
     static_assert(THREADS >= RADIX, "one thread per digit in the scan phases");
 
     // plain pointer arithmetic on the shared array keeps the shared address space (LDS/STS, 32-bit addresses)
@@ -364,7 +372,7 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
             if (!full_tile && tid == RADIX - 1) pub -= (u32)TILE - tile_valid;      // padding is not data
             st_relaxed_u32(my_status, pub | (ti.idx == 0 ? FLAG_INCL : FLAG_PARTIAL));
             if (SEG) {
-                // inside a segment the predecessor finished a wave of CTAs ago: one load nearly always finds its inclusive prefix
+                // a group's first tile: the predecessor finished a wave of CTAs ago, one load nearly always finds its inclusive prefix
                 lbv[0] = ti.idx > 0 ? ld_relaxed_u32(my_status - RADIX) : FLAG_INCL;
             }
             else {
@@ -429,8 +437,8 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
                     bool done = false;
                     u32 v[LB];
                     if (SEG) {
-                        // fast path: the prefetched predecessor carries an inclusive prefix.  Otherwise (tiles of a dominant segment that
-                        // run at the same time) continue with batches of LB predecessors per round trip.
+                        // fast path: the prefetched predecessor carries an inclusive prefix.  Otherwise (the other members of a group,
+                        // tiles of a dominant segment that run at the same time) continue with batches of LB predecessors per round trip.
                         if (lbv[0] & FLAG_INCL) { excl = lbv[0] & VALUE_MASK; done = true; }
                         else {
                             v[0] = lbv[0];

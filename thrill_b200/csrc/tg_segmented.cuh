@@ -1,11 +1,14 @@
-// tg_segmented.cuh — partition passes without a chained scan between tiles that run at the same time.
+// tg_segmented.cuh — partition passes whose chained scan spans a few tiles that run at the same time, not a whole wave.
 //
 // A partition pass needs, for every tile and digit, the number of items with that digit in the tiles before it.
 // The chained scan ("decoupled look-back", tg_partition.cuh) gets it from the tiles themselves, which makes every tile
 // wait for the tiles processed at the same time on the other SMs.  Both forms below
-// know the bases of coarse SEGMENTS up front and list the tiles so that consecutive tiles of the processing order
-// belong to different segments; the scan chain of a tile only spans its own segment and its predecessor finished a
-// whole wave of CTAs earlier:
+// know the bases of coarse SEGMENTS up front, so the scan chain of a tile only spans its own segment, and list the tiles
+// in rounds of groups: round q holds the q-th group of TILE_GROUP (G) neighbouring tiles of every segment.  The G tiles of
+// a group run in the same wave of CTAs and write each digit's runs next to each other in memory; the predecessor of a
+// group's first tile finished a whole wave earlier, and a later member waits at most for the members before it, which
+// publish their counts right after ranking.  Every tile's predecessors come earlier in the list, and every CTA takes its
+// tiles in list order, so the scan always makes progress.
 //   * chunked pass   — any input: cut it into contiguous chunks, one counting read gives segbase[chunk][digit]
 //   * segmented pass — input already partitioned by a more significant digit: the buckets are the segments, items never
 //     leave their bucket, and one counting read serves every further pass inside the buckets.
@@ -198,11 +201,13 @@ static __global__ void seg_scan_kernel(const u32* __restrict__ segcount, const u
     segbase[((size_t)pos * nseg + seg) * RADIX + d] = add + incl - c;
 }
 
-// Tile list of `nseg` segments of seg_size[] items laid out back to back, interleaving the segments: round r holds the
-// r-th tile of every segment that has one (so a tile's predecessor in its segment is a whole round away).  The list is
-// staged in pinned host buffer `stage` (0/1; the list staged there before must have been consumed by its copy: callers
-// alternate the two buffers between stream synchronisations) and copied to *d_tiles (workspace slot `ws_slot`).
+// Tile list of `nseg` segments of seg_size[] items laid out back to back, interleaving groups of G = TILE_GROUP tiles of the
+// segments: round q holds tiles [G*q, G*q + G) of every segment that has them (fewer in a segment's last round), one
+// segment's group after the other, segments ordered by tile count (descending, ties by index).  The list is staged in pinned
+// host buffer `stage` (0/1; the list staged there before must have been consumed by its copy: callers alternate the two
+// buffers between stream synchronisations) and copied to *d_tiles (workspace slot `ws_slot`).
 inline int build_tile_list(tg_ctx* ctx, int nseg, const u32* seg_size, u32 tile, int stage, int ws_slot, uint4** d_tiles, u32* total_out) {
+    constexpr u32 G = TILE_GROUP;
     if (nseg > 4096) return tg_set_error(ctx, TG_ERR_ARG, "tile list: at most 4096 segments");
     std::vector<u32> ntiles(nseg), row0(nseg), start(nseg), order(nseg);
     u32 total = 0, acc = 0, maxt = 0;
@@ -220,13 +225,16 @@ inline int build_tile_list(tg_ctx* ctx, int nseg, const u32* seg_size, u32 tile,
     uint4* h_tiles;
     TG_TRY(tg_pinned_list(ctx, stage, (size_t)total * sizeof(uint4) + 16, (void**)&h_tiles));
     u32 w = 0;
-    for (u32 r = 0; r < maxt; ++r) {
+    for (u32 r0 = 0; r0 < maxt; r0 += G) {
         for (int o = 0; o < nseg; ++o) {
             const u32 sg = order[o];
-            if (ntiles[sg] <= r) break;               // sorted by tile count: nobody further has a round r
-            const u32 off = r * tile;
-            const u32 len = seg_size[sg] - off < tile ? seg_size[sg] - off : tile;
-            h_tiles[w++] = make_uint4(start[sg] + off, len, row0[sg] + r, (sg << 20) | r);
+            if (ntiles[sg] <= r0) break;              // sorted by tile count: nobody further has a tile in this round
+            const u32 r1 = ntiles[sg] - r0 < G ? ntiles[sg] : r0 + G;
+            for (u32 r = r0; r < r1; ++r) {
+                const u32 off = r * tile;
+                const u32 len = seg_size[sg] - off < tile ? seg_size[sg] - off : tile;
+                h_tiles[w++] = make_uint4(start[sg] + off, len, row0[sg] + r, (sg << 20) | r);
+            }
         }
     }
     TG_TRY(tg_ws_get(ctx, ws_slot, (size_t)total * sizeof(uint4) + 16, (void**)d_tiles));
@@ -238,8 +246,11 @@ inline int build_tile_list(tg_ctx* ctx, int nseg, const u32* seg_size, u32 tile,
 // ---- the same interleaved tile list for the RADIX buckets of a pass, built on the device (no host round trip) ----------------
 // aux (RADIX * 4 + 8 words): row0[s] (first status row of segment s) | sortrank[s] (position of s when the segments are ordered
 // by tile count, descending) | snt[k] (tile counts in that order) | P[k] (prefix sums of snt, RADIX + 1 entries) | total.
-// Round r of the list holds the r-th tile of every segment that has one, in sorted order: the position of tile (s, r) is
-// A(r) + sortrank[s] with A(r) = sum over segments of min(tiles, r) = r * C(r) + (total - P[C(r)]), C(r) = #segments with > r tiles.
+// Round q of the list holds tiles [g0, g0 + G) (g0 = G * q) of every segment that has them, segments in sorted order.  Tile
+// (s, r) of round q sits at A(g0) + B(s) + (r - g0):
+//   A(g0) = tiles of the earlier rounds = sum over segments of min(tiles, g0) = g0 * C + (total - P[C]), C = #segments with > g0 tiles;
+//   B(s)  = tiles of this round of the segments sorted before s (k = sortrank[s] of them, all with > g0 tiles): the first F of
+//           them (F = #segments with >= g0 + G tiles) have G each, the others snt[i] - g0:  G * min(k, F) + (P[k] - P[F]) - g0 * (k - F).
 static __global__ void __launch_bounds__(RADIX) seg_tiles_prepare_kernel(const u32* __restrict__ seg_size, u32 tile, int drop_last,
                                                                          u32* __restrict__ aux, u32* __restrict__ total_out) {
     __shared__ u32 nt[RADIX], incl[RADIX], snt[RADIX];
@@ -287,10 +298,15 @@ static __global__ void __launch_bounds__(256) seg_tiles_fill_kernel(const u32* _
     int lo = 0, hi = RADIX;                    // last segment with row0 <= row that has tiles
     while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (row0[mid] <= row) lo = mid; else hi = mid; }
     const u32 sg = (u32)lo, r = row - row0[sg];
-    int c0 = 0, c1 = RADIX;                    // C(r) = number of entries of the descending snt that are > r
-    while (c0 < c1) { const int mid = (c0 + c1) >> 1; if (snt[mid] > r) c0 = mid + 1; else c1 = mid; }
-    const u32 C = (u32)c0;
-    const u32 pos = r * C + (total - P[C]) + srank[sg];
+    auto count_above = [&](u32 x) -> u32 {     // number of entries of the descending snt that are > x
+        int c0 = 0, c1 = RADIX;
+        while (c0 < c1) { const int mid = (c0 + c1) >> 1; if (snt[mid] > x) c0 = mid + 1; else c1 = mid; }
+        return (u32)c0;
+    };
+    const u32 g0 = r - r % TILE_GROUP;         // first tile of the round
+    const u32 C = count_above(g0), F = count_above(g0 + TILE_GROUP - 1), k = srank[sg];
+    const u32 before = k <= F ? TILE_GROUP * k : TILE_GROUP * F + (P[k] - P[F]) - g0 * (k - F);
+    const u32 pos = g0 * C + (total - P[C]) + before + (r - g0);
     const u32 size = (drop_last && sg == RADIX - 1) ? 0u : seg_size[sg];
     const u32 off = r * tile;
     tiles[pos] = make_uint4(seg_start[sg] + off, size - off < tile ? size - off : tile, row, (sg << 20) | r);
