@@ -20,8 +20,9 @@
  * _file / _dev forms) takes at most 2^30 - 1 items per call and worker (n_local), and a worker receives at most 2^30 - 1
  * items in an exchange: the partition passes count in 30-bit fields.  ReduceToIndex gives each worker fewer than 2^31
  * indices of the result.  Merge (tg_merge and its forms) takes at most 2^30 - 1 items in a worker's k inputs together, and gives
- * each worker at most 2^30 - 1 items of the result; it merges 2..16 inputs of 8- or 16-byte items.  The collective operators
- * return TG_ERR_TOO_LARGE on every rank or on none.
+ * each worker at most 2^30 - 1 items of the result; it merges 2..16 inputs of 8- or 16-byte items.  InnerJoin (tg_inner_join
+ * and its _file form) takes at most 2^30 - 1 items per worker and side, before and after its exchange, and gives each worker at
+ * most 2^30 - 1 items of the result.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
  ******************************************************************************/
 #ifndef THRILL_GPU_H
 #define THRILL_GPU_H
@@ -120,7 +121,8 @@ uint64_t tg_hot_records(const tg_ctx* ctx);
  * and the number of launches of `kernel_class` since tg_profile_enable(ctx, 1). */
 enum { TG_K_RADIX_HIST = 0, TG_K_PARTITION = 1, TG_K_MERGE = 2, TG_K_PREAGG = 3, TG_K_AGGREGATE = 4,
        TG_K_COMPACT = 5, TG_K_OTHER = 6, TG_K_FIXUP = 7, TG_K_SEGCOUNT = 8,
-       TG_K_EXCHANGE = 9 /* the NCCL Alltoallv (not a kernel of ours: timed like one) */, TG_K_NUM = 10 };
+       TG_K_EXCHANGE = 9 /* the NCCL Alltoallv (not a kernel of ours: timed like one) */,
+       TG_K_JOIN = 10 /* InnerJoin's co-rank count, offset scan and emit kernels */, TG_K_NUM = 11 };
 int tg_profile_enable(tg_ctx* ctx, int on);
 int tg_profile_get(tg_ctx* ctx, int kernel_class, float* out_total_ms, uint64_t* out_launches);
 /* the individual launch durations of `kernel_class` in launch order (up to `capacity`); *out_n = how many there are */
@@ -308,6 +310,36 @@ int tg_merge_select(tg_ctx* ctx, const tg_key_desc* desc, const void* const* d_r
  * outside [sum(less), sum(less + equal)], or bounds of a run decreasing in d. */
 int tg_merge_plan(uint32_t p, uint32_t k, const uint64_t* targets, const uint64_t* less, const uint64_t* equal,
                   uint64_t* out_bounds);
+
+/* ---- InnerJoin: DIA<pair<u64, V1>> ⋈ DIA<pair<u64, V2>> on .first (api::InnerJoin, api/inner_join.hpp:700-830) ---------------------
+ * Both inputs are 16-byte items (uint64_t key, 8-byte value: any type, copied as bits).  Every pair (l, r) with l.first == r.first
+ * gives one output item, by join_fn:
+ *   TG_JOIN_KEY_VALUES  std::tuple<uint64_t, V1, V2> = (key, l.second, r.second), 24 bytes: serialized member by member in get<0..2>
+ *                       order (data/serialization.hpp:89-178), so the device layout is (key, v1, v2)
+ *   TG_JOIN_VALUES      std::pair<V1, V2> = (l.second, r.second), 16 bytes
+ * Placement: worker Hash128to64(0, key) % p owns a key (as in ReduceByKey).  The reference's JoinNode (:61-481) exchanges both
+ * sides by that hash, sorts each side locally and joins by a sort-merge on the host; here each side goes through one exchange
+ * (the partition pass storing into the owners' windows), a stable local radix sort by the key, then a co-rank count (merge path
+ * over left and right), an exclusive scan of the match counts and a load-balanced emit kernel (each CTA a range of the output).
+ * Order within a worker: ascending key, then the left item's global position, then the right item's (global position = position
+ * in the concatenation of the workers' shards).  This is one of the outcomes the reference allows; it leaves equal keys unordered
+ * and, with location detection, may place keys elsewhere, so comparisons with it are on the multiset.  Key 0 is an ordinary key.
+ * Inputs are read, never modified; an empty side gives an empty result.  item_bytes other than 16 or an unknown join_fn is
+ * TG_ERR_ARG.  The largest output count of any worker is agreed on (all-reduce) before output memory is allocated, so an output of
+ * 2^30 or more items on any worker is TG_ERR_TOO_LARGE on every rank.  Host round trips: with p > 1 three (the two count matrices
+ * of the exchanges and the output-size all-reduce), with p = 1 one (the output size).  Collective. */
+enum { TG_JOIN_KEY_VALUES = 0, TG_JOIN_VALUES = 1 };
+typedef struct {
+    uint32_t item_bytes;       /* 16, both inputs */
+    uint32_t join_fn;          /* TG_JOIN_* */
+} tg_join_desc;
+/* device buffers; *out_dptr as for tg_sort (ctx-owned, valid until the next operator call).  Collective. */
+int tg_inner_join(tg_ctx* ctx, const tg_join_desc* desc, const void* d_left, size_t n_left, const void* d_right, size_t n_right,
+                  void** out_dptr, size_t* out_n);
+/* the drop-in call (GpuJoinNode::Execute): each side a host File (Blocks) or a device File (read in place, left intact); the
+ * result is fetched with tg_fetch_output or taken with tg_output_detach (item_bytes 24 or 16) */
+int tg_inner_join_file(tg_ctx* ctx, const tg_join_desc* desc, const tg_merge_input* left, const tg_merge_input* right,
+                       size_t* out_items);
 
 /* ---- synthetic inputs of SURVEY.md §8(d), generated on the device (bench / tests support) ------------ */
 int tg_gen_sort_uniform(tg_ctx* ctx, void* d_out, uint64_t begin, uint64_t n, uint64_t seed);

@@ -7,6 +7,7 @@ Mirrors (same names, argument meaning and error behaviour) the slice of thrill/a
     DIA<T>::ReducePair(reduce_fn)          thrill/api/reduce_by_key.hpp:410-449
     DIA<T>::ReduceByKey(key_ex, reduce_fn) thrill/api/reduce_by_key.hpp:312-363
     DIA<T>::Merge(second, cmp) / api::Merge thrill/api/merge.hpp:674-721
+    api::InnerJoin(l, r, key1, key2, fn)   thrill/api/inner_join.hpp:700-827
     DIA<T>::Size / AllGather / Gather      thrill/api/size.hpp, all_gather.hpp, gather.hpp
 A DIA here holds its local shard as a host numpy array — the stand-in for a data::File whose Blocks are
 1 MiB ByteBlocks (data/byte_block.cpp:23-24, data/block_writer.hpp:405-420).  Operators hand the Blocks to the
@@ -47,6 +48,11 @@ MinDouble = _Functor("min<double>", capi.OP_MIN_F64)
 MaxDouble = _Functor("max<double>", capi.OP_MAX_F64)
 First = _Functor("first", capi.OP_FIRST)
 KeyIsFirst = _Functor("pair.first")                       # the key extractor ReducePair builds (:444-449)
+# recognised join functions of InnerJoin on pair DIAs
+JoinKeyValues = _Functor("(l, r) -> tuple(l.first, l.second, r.second)", capi.JOIN_KEY_VALUES)
+JoinValues = _Functor("(l, r) -> pair(l.second, r.second)", capi.JOIN_VALUES)
+KEY_V1_V2 = np.dtype([("key", "<u8"), ("v1", "<u8"), ("v2", "<u8")])     # std::tuple<uint64_t, V1, V2>, member-wise
+V1_V2 = np.dtype([("v1", "<u8"), ("v2", "<u8")])                         # std::pair<V1, V2>
 
 
 def bind_to_gpu_numa_node(device):
@@ -166,6 +172,34 @@ def Merge(compare_function, *dias, **kw):
     tg = first.ctx.tg
     tg.ck(tg.L.tg_merge_file(tg.h, C.byref(desc), inputs, len(dias), C.byref(n_out)))
     return DIA(first.ctx, first._fetch(n_out.value, dtype, desc.item_bytes, kw.get("_pinned_out")))
+
+
+def InnerJoin(first, second, key_extractor1, key_extractor2, join_function, **kw):
+    """api::InnerJoin(left, right, key_extractor1, key_extractor2, join_function) (api/inner_join.hpp:700-827) on two DIAs of
+    pair<uint64_t, 8-byte value> joined on .first: JoinKeyValues gives KEY_V1_V2 items, JoinValues V1_V2 items.  Worker
+    Hash128to64(0, key) % p holds a key's results, ordered by (key, left global position, right global position)."""
+    if key_extractor1 is not KeyIsFirst or key_extractor2 is not KeyIsFirst:
+        raise capi.ThrillGpuError("InnerJoin: only the pair.first key extractors are recognised by the GPU path")
+    if join_function not in (JoinKeyValues, JoinValues):
+        raise capi.ThrillGpuError("InnerJoin: join function %r is not one the GPU path recognises" % (join_function,))
+    if first.ctx is not second.ctx:
+        raise capi.ThrillGpuError("InnerJoin: the DIAs belong to different contexts")
+    for d in (first, second):
+        if not (d.items.ndim == 1 and d.items.dtype == KV):
+            raise capi.ThrillGpuError("InnerJoin: items must be pair<uint64_t, 8-byte value>")
+    desc = capi.JoinDesc(16, join_function.code)
+    sides = (capi.MergeInput * 2)()
+    keep = []
+    for j, d in enumerate((first, second)):
+        blocks, nb = d._blocks(d.items)
+        keep.append(blocks)
+        sides[j].blocks = C.cast(blocks, C.POINTER(capi.Block))
+        sides[j].nblocks = nb
+    n_out = C.c_size_t()
+    tg = first.ctx.tg
+    tg.ck(tg.L.tg_inner_join_file(tg.h, C.byref(desc), C.byref(sides[0]), C.byref(sides[1]), C.byref(n_out)))
+    dtype = KEY_V1_V2 if join_function is JoinKeyValues else V1_V2
+    return DIA(first.ctx, first._fetch(n_out.value, dtype, dtype.itemsize, kw.get("_pinned_out")))
 
 
 class DIA(object):

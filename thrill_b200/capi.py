@@ -12,7 +12,8 @@ LIB_PATH = os.environ.get("TG_LIB") or os.path.join(HERE, "csrc", "libthrill_gpu
 TG_OK = 0
 KEY_UINT_LE, KEY_BYTES_BE = 0, 1
 OP_SUM_F64, OP_SUM_U64, OP_MIN_U64, OP_MAX_U64, OP_MIN_F64, OP_MAX_F64, OP_FIRST = range(7)
-K_RADIX_HIST, K_PARTITION, K_MERGE, K_PREAGG, K_AGGREGATE, K_COMPACT, K_OTHER, K_FIXUP, K_SEGCOUNT, K_EXCHANGE = range(10)
+K_RADIX_HIST, K_PARTITION, K_MERGE, K_PREAGG, K_AGGREGATE, K_COMPACT, K_OTHER, K_FIXUP, K_SEGCOUNT, K_EXCHANGE, K_JOIN = range(11)
+JOIN_KEY_VALUES, JOIN_VALUES = 0, 1
 
 
 class KeyDesc(C.Structure):
@@ -35,6 +36,10 @@ class DevFile(C.Structure):
 class MergeInput(C.Structure):
     """tg_merge_input: a device File (dev) or a host File (blocks, nblocks)"""
     _fields_ = [("dev", C.POINTER(DevFile)), ("blocks", C.POINTER(Block)), ("nblocks", C.c_size_t)]
+
+
+class JoinDesc(C.Structure):
+    _fields_ = [("item_bytes", C.c_uint32), ("join_fn", C.c_uint32)]
 
 
 class BlockGeom(C.Structure):
@@ -112,6 +117,8 @@ SYMBOLS = [
     ("tg_merge_file", _i, [_vp, _P(KeyDesc), _P(MergeInput), _u32, _P(_sz)]),
     ("tg_merge_select", _i, [_vp, _P(KeyDesc), _P(_vp), _P(_sz), _u32, _u32, _P(_u64)]),
     ("tg_merge_plan", _i, [_u32, _u32, _P(_u64), _P(_u64), _P(_u64), _P(_u64)]),
+    ("tg_inner_join", _i, [_vp, _P(JoinDesc), _vp, _sz, _vp, _sz, _P(_vp), _P(_sz)]),
+    ("tg_inner_join_file", _i, [_vp, _P(JoinDesc), _P(MergeInput), _P(MergeInput), _P(_sz)]),
     ("tg_transfer_bytes", _i, [_vp, _P(_u64), _P(_u64)]),
     ("tg_gen_sort_uniform", _i, [_vp, _vp, _u64, _u64, _u64]),
     ("tg_gen_reduce_uniform", _i, [_vp, _vp, _u64, _u64, _u64, _u64, _i]),

@@ -193,6 +193,27 @@ void xchg_recv_offsets(tg_ctx* ctx, u64* before) {
     tg_exchange_plan((u32)ctx->nranks, (u32)ctx->rank, h_mat, (uint64_t*)sc, (uint64_t*)rc, (uint64_t*)before, (uint64_t*)&nr, (uint64_t*)&worst);
 }
 
+int evacuate_window_inputs(tg_ctx* ctx, const void** in, const size_t* bytes, uint32_t k) {
+    const char* b = (const char*)ctx->xwin.base;
+    if (!b) return TG_OK;
+    const char *lo = nullptr, *hi = nullptr;
+    for (uint32_t j = 0; j < k; ++j) {
+        const char* q = (const char*)in[j];
+        if (!bytes[j] || q < b || q >= b + ctx->xwin.cap) continue;
+        if (!lo || q < lo) lo = q;
+        if (!hi || q + bytes[j] > hi) hi = q + bytes[j];
+    }
+    if (!lo) return TG_OK;
+    char* d;
+    TG_TRY(tg_ws_get(ctx, WS_AUX, (size_t)(hi - lo) + 16, (void**)&d));
+    TG_CUDA(ctx, cudaMemcpyAsync(d, lo, (size_t)(hi - lo), cudaMemcpyDeviceToDevice, ctx->stream));
+    for (uint32_t j = 0; j < k; ++j) {
+        const char* q = (const char*)in[j];
+        if (bytes[j] && q >= lo && q < hi) in[j] = d + (q - lo);
+    }
+    return TG_OK;
+}
+
 void xwin_release(tg_ctx* ctx) {
     unmap_peers(ctx);
     if (ctx->xwin.base) cudaFree(ctx->xwin.base);

@@ -34,6 +34,20 @@ int xwin_barrier(tg_ctx* ctx);                                      // stream-or
 int xchg_counts(tg_ctx* ctx, const u32* d_totals, int item_bytes, XchgResult* res, u64* need_bytes_max);
 int xchg_upload_dest(tg_ctx* ctx, int item_bytes, const XchgResult& res, void*** d_dbase_out);
 void xchg_recv_offsets(tg_ctx* ctx, u64* before);                  // before[d] = items of the lower ranks in worker d's window
+// inputs that lie inside the exchange window (an un-detached result of the previous collective operator) are moved out of
+// the peers' way first (into WS_AUX): the span they cover is copied once, so that inputs sharing it stay consistent
+int evacuate_window_inputs(tg_ctx* ctx, const void** in, const size_t* bytes, uint32_t k);
+
+// destination worker of a 16-byte (u64 key, value) item: Hash128to64(0, key) % p (core/reduce_functional.hpp:60-72), the
+// owner of a key in ReduceByKey and InnerJoin
+struct HashDigit {
+    u32 p;
+    static constexpr bool kStoreDigit = true;
+    static constexpr bool kHasDrop = false;
+    static constexpr int kScratch = 0;
+    __device__ __forceinline__ void init() {}
+    __device__ __forceinline__ u32 operator()(const ulonglong2& v, u32) const { return (u32)(hash128to64_dev(0, v.x) % p); }
+};
 
 // Stable partition of n local items by fn (destination worker, < p) + Alltoallv.  Collective.
 // n >= 2^30 (over the per-call limit): this rank sends nothing and reports 2^30 items for worker 0 in its counts, so that

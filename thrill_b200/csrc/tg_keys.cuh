@@ -82,6 +82,20 @@ inline int make_key_view(const tg_key_desc* d, KeyView* kv) {
     return TG_OK;
 }
 
+// merge path of sorted A and B: the number of A items among the first `diag` merged outputs, ties to A (stable).  Used by the
+// merges (tg_merge.cu) and by the join's co-ranks (tg_join.cu).
+template <class Item>
+__device__ __forceinline__ u32 merge_path_search(const Item* A, u32 na, const Item* B, u32 nb, u32 diag, const KeyView& kv) {
+    u32 lo = diag > nb ? diag - nb : 0, hi = diag < na ? diag : na;
+    while (lo < hi) {
+        u32 mid = (lo + hi) >> 1;            // take mid+1 items from A?
+        Canon a = canon_key(A[mid], kv);
+        Canon b = canon_key(B[diag - 1 - mid], kv);
+        if (canon_less(b, a)) hi = mid; else lo = mid + 1;      // A[mid] <= B[..] -> A first (stable)
+    }
+    return lo;
+}
+
 // tg_merge.cu: stable merge of k sorted runs of 8- or 16-byte items into d_out (d_tmp: scratch of the same size), ties to the
 // lower run index
 int merge_runs(tg_ctx* ctx, const KeyView& kv, uint32_t item_bytes, const void* const* runs, const uint64_t* run_items,

@@ -26,19 +26,6 @@ namespace {
 constexpr int MG_THREADS = 256;
 template <int WORDS> struct MergeCfg { static constexpr int VT = 16 / WORDS; static constexpr int TILE = MG_THREADS * VT; };
 
-template <class Item>
-__device__ __forceinline__ u32 merge_path_search(const Item* A, u32 na, const Item* B, u32 nb, u32 diag, const KeyView& kv) {
-    // number of A items among the first `diag` merged outputs
-    u32 lo = diag > nb ? diag - nb : 0, hi = diag < na ? diag : na;
-    while (lo < hi) {
-        u32 mid = (lo + hi) >> 1;            // take mid+1 items from A?
-        Canon a = canon_key(A[mid], kv);
-        Canon b = canon_key(B[diag - 1 - mid], kv);
-        if (canon_less(b, a)) hi = mid; else lo = mid + 1;      // A[mid] <= B[..] -> A first (stable)
-    }
-    return lo;
-}
-
 // split[t] = number of A items among the first min(t * TILE, na + nb) outputs, t = 0..ntiles.  On sorted runs the splits
 // partition A and B; on unsorted ones they may not, and *bad is set: the merge then concatenates A and B instead, so that
 // its output is still a permutation of its input.
@@ -356,29 +343,6 @@ __global__ void __launch_bounds__(256) copy_words_kernel(const u64* __restrict__
             if (ok1) q[1] = v1;
         }
     }
-}
-
-// inputs that lie inside the exchange window (an un-detached result of the previous collective operator) are moved out of
-// the peers' way first: the span they cover is copied once, so that inputs sharing it stay consistent
-int evacuate_window_inputs(tg_ctx* ctx, const void** in, const size_t* bytes, uint32_t k) {
-    const char* b = (const char*)ctx->xwin.base;
-    if (!b) return TG_OK;
-    const char *lo = nullptr, *hi = nullptr;
-    for (uint32_t j = 0; j < k; ++j) {
-        const char* q = (const char*)in[j];
-        if (!bytes[j] || q < b || q >= b + ctx->xwin.cap) continue;
-        if (!lo || q < lo) lo = q;
-        if (!hi || q + bytes[j] > hi) hi = q + bytes[j];
-    }
-    if (!lo) return TG_OK;
-    char* d;
-    TG_TRY(tg_ws_get(ctx, WS_AUX, (size_t)(hi - lo) + 16, (void**)&d));
-    TG_CUDA(ctx, cudaMemcpyAsync(d, lo, (size_t)(hi - lo), cudaMemcpyDeviceToDevice, ctx->stream));
-    for (uint32_t j = 0; j < k; ++j) {
-        const char* q = (const char*)in[j];
-        if (bytes[j] && q >= lo && q < hi) in[j] = d + (q - lo);
-    }
-    return TG_OK;
 }
 
 template <int WORDS>

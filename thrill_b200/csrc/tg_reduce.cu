@@ -172,16 +172,6 @@ compact_kernel(const ulonglong2* __restrict__ tab, u64 cap, ulonglong2* __restri
     }
 }
 
-// destination worker of an item: Hash128to64(0, key) % p  (core/reduce_functional.hpp:60-72)
-struct HashDigit {
-    u32 p;
-    static constexpr bool kStoreDigit = true;
-    static constexpr bool kHasDrop = false;
-    static constexpr int kScratch = 0;
-    __device__ __forceinline__ void init() {}
-    __device__ __forceinline__ u32 operator()(const ulonglong2& v, u32) const { return (u32)(key_hash(v.x) % p); }
-};
-
 struct ReduceScratch {
     u64* cursor;        // [0] output cursor
     u64* zero_slot;     // [0] flag, [1] value

@@ -6,6 +6,7 @@
  *     thrill_gpu::Sort(dia [, std::less<T>/std::greater<T>])     <->  DIA<T>::Sort      (api/sort.hpp:800)
  *     thrill_gpu::ReducePair(dia, std::plus<double> ...)          <->  DIA<T>::ReducePair(api/reduce_by_key.hpp:410)
  *     thrill_gpu::Merge(std::less<T>(), dia0, dia1, ...)          <->  api::Merge        (api/merge.hpp:673)
+ *     thrill_gpu::InnerJoin(l, r, KeyFirst(), KeyFirst(), JoinValues()) <->  api::InnerJoin (api/inner_join.hpp:700)
  * Everything else of the pipeline (sources, LOps, other DOps, actions, the net/data layers) is the
  * UNMODIFIED reference library: this header only includes it.  The heavy lifting happens behind the C ABI
  * of include/thrill_gpu.h (libthrill_gpu.so): the nodes hand the Blocks of their input data::File to
@@ -36,6 +37,7 @@
 #include <cstring>
 #include <functional>
 #include <memory>
+#include <tuple>
 #include <type_traits>
 #include <utility>
 #include <vector>
@@ -189,6 +191,35 @@ struct OnSecond {
     ValueFunction fn;
     template <typename P>
     P operator () (const P& a, const P& b) const { return P(a.first, fn(a.second, b.second)); }
+};
+
+//! The join functions thrill_gpu::InnerJoin recognises (api::InnerJoin takes any function of (left item, right item),
+//! api/inner_join.hpp:700-827), on pair<uint64_t, V1> and pair<uint64_t, V2> joined on .first.  They are plain functors, so the
+//! stock api::InnerJoin takes them too.
+struct JoinKeyValues {
+    template <typename L, typename R>
+    std::tuple<uint64_t, typename L::second_type, typename R::second_type> operator () (const L& l, const R& r) const {
+        return std::make_tuple(l.first, l.second, r.second);
+    }
+};
+struct JoinValues {
+    template <typename L, typename R>
+    std::pair<typename L::second_type, typename R::second_type> operator () (const L& l, const R& r) const {
+        return std::make_pair(l.second, r.second);
+    }
+};
+//! out_bytes: the SERIALIZED output item size (std::tuple is written member by member, data/serialization.hpp:89-178)
+template <typename JoinFunction>
+struct JoinDesc { static constexpr bool supported = false; };
+template <>
+struct JoinDesc<JoinKeyValues>{
+    static constexpr bool supported = true;
+    static constexpr uint32_t fn = TG_JOIN_KEY_VALUES, out_bytes = 24;
+};
+template <>
+struct JoinDesc<JoinValues>{
+    static constexpr bool supported = true;
+    static constexpr uint32_t fn = TG_JOIN_VALUES, out_bytes = 16;
 };
 
 /******************************************************************************/
@@ -586,6 +617,106 @@ private:
     bool have_host_file_ = false;
 };
 
+//! api::InnerJoin (api/inner_join.hpp:700-827): the JoinNode protocol (one File per parent, registered with
+//! AddChild(this, chain, index), :133-157; StopPreOp per parent) with the hash exchange, the local sorts and the join of
+//! Execute / PushData (:159-312) behind tg_inner_join_file.  Either side may arrive as a device File from a parent GPU node.
+//! kOutBytes: the serialized size of ValueType (24 for the (key, v1, v2) tuple, 16 for the (v1, v2) pair).
+template <typename ValueType, typename LeftType, typename RightType, uint32_t kOutBytes>
+class GpuJoinNode final : public thrill::api::DOpNode<ValueType>, public GpuNodeBase
+{
+    using Super = thrill::api::DOpNode<ValueType>;
+    using Super::context_;
+
+public:
+    template <typename LeftDIA, typename RightDIA>
+    GpuJoinNode(const LeftDIA& left, const RightDIA& right, const tg_join_desc& desc)
+        : Super(left.ctx(), "GpuInnerJoin", { left.id(), right.id() }, { left.node(), right.node() }),
+          desc_(desc), parent_stack_empty_({ { LeftDIA::stack_empty, RightDIA::stack_empty } }) {
+        for (size_t i = 0; i < 2; ++i) {
+            files_[i] = context_.GetFilePtr(this);
+            writers_[i] = files_[i]->GetWriter();
+        }
+        thrill::data::File::Writer* w0 = &writers_[0];
+        thrill::data::File::Writer* w1 = &writers_[1];
+        auto pre_op_fn0 = [w0](const LeftType& input) { w0->Put(input); };
+        auto pre_op_fn1 = [w1](const RightType& input) { w1->Put(input); };
+        left.node()->AddChild(this, left.stack().push(pre_op_fn0).fold(), 0);
+        right.node()->AddChild(this, right.stack().push(pre_op_fn1).fold(), 1);
+    }
+
+    bool OnPreOpFile(const thrill::data::File& file, size_t parent_index) final {
+        if (!parent_stack_empty_[parent_index]) return false;
+        *files_[parent_index] = file.Copy();
+        return true;
+    }
+
+    bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes, size_t parent_index) final {
+        if (!parent_stack_empty_[parent_index] || item_bytes != 16) return false;
+        device_inputs_[parent_index] = file;
+        return true;
+    }
+
+    void StopPreOp(size_t parent_index) final { writers_[parent_index].Close(); }
+
+    DIAMemUse ExecuteMemUse() final { return DIAMemUse::Max(); }
+
+    //! both exchanges, the local sorts and the join behind tg_inner_join_file.  Collective.  The result stays in HBM.
+    void Execute() final {
+        tg_ctx* c = WorkerCtx(context_);
+        std::vector<std::unique_ptr<PinnedFileView> > views;
+        std::array<tg_merge_input, 2> in;
+        for (size_t i = 0; i < 2; ++i) {
+            if (device_inputs_[i]) {
+                in[i] = tg_merge_input { device_inputs_[i]->get(), nullptr, 0 };
+                continue;
+            }
+            views.emplace_back(new PinnedFileView(*files_[i], context_.local_worker_id()));
+            in[i] = tg_merge_input { nullptr, views.back()->data(), views.back()->size() };
+        }
+        size_t out_items = 0;
+        Check(c, tg_inner_join_file(c, &desc_, &in[0], &in[1], &out_items), "tg_inner_join_file");
+        views.clear();
+        for (size_t i = 0; i < 2; ++i) {
+            files_[i]->Clear();
+            device_inputs_[i].reset();
+        }
+        tg_dev_file f;
+        Check(c, tg_output_detach(c, &f), "tg_output_detach");
+        device_result_ = std::make_shared<DeviceFile>(c, f);
+        have_host_file_ = false;
+    }
+
+    DIAMemUse PushDataMemUse() final { return 0; }
+
+    //! GPU children take the result in HBM (a 16-byte JoinValues result can feed thrill_gpu::ReducePair); a host File is
+    //! written only if another kind of child needs one
+    void PushData(bool consume) final {
+        if (device_result_ && AllChildrenAreGpuNodes(*this)) {
+            bool all = true;
+            for (const auto& ch : this->children_)
+                all = dynamic_cast<GpuNodeBase*>(ch.node)->OnPreOpDeviceFile(device_result_, kOutBytes, ch.parent_index) && all;
+            if (all) return;
+        }
+        if (!have_host_file_) {
+            FetchDeviceFileIntoFile(WorkerCtx(context_), context_, *device_result_, kOutBytes, joined_file_);
+            have_host_file_ = true;
+        }
+        this->PushFile(joined_file_, consume);
+    }
+
+    void Dispose() final { joined_file_.Clear(); device_result_.reset(); have_host_file_ = false; }
+
+private:
+    tg_join_desc desc_;
+    const std::array<bool, 2> parent_stack_empty_;
+    thrill::data::FilePtr files_[2];
+    thrill::data::File::Writer writers_[2];
+    std::array<DeviceFilePtr, 2> device_inputs_;
+    thrill::data::File joined_file_ { context_.GetFile(this) };
+    DeviceFilePtr device_result_;
+    bool have_host_file_ = false;
+};
+
 /******************************************************************************/
 // front doors (same argument meaning as DIA<T>::Sort / DIA<T>::ReducePair)
 
@@ -672,6 +803,34 @@ auto Merge(const Comparator& /* comparator */, const FirstDIA& first_dia, const 
     tlx::vexpand((dias.AssertValid(), 0) ...);
     auto node = tlx::make_counting<GpuMergeNode<ValueType, 1 + sizeof ... (DIAs)> >(
         SortDesc<ValueType, Comparator>::make(), first_dia, dias ...);
+    return DIA<ValueType>(node);
+}
+
+//! api::InnerJoin(left, right, key_extractor1, key_extractor2, join_function) (api/inner_join.hpp:700-827) for pair DIAs joined on
+//! .first: left = DIA<pair<uint64_t, V1>>, right = DIA<pair<uint64_t, V2>> with 8-byte V1 and V2, key extractors KeyFirst,
+//! join_function JoinKeyValues (-> tuple<uint64_t, V1, V2>) or JoinValues (-> pair<V1, V2>).  Worker Hash128to64(0, key) % p
+//! holds a key's results, ordered by (key, left global position, right global position), one of the orders the stock operator
+//! allows.  InnerJoin(a, a, ...) is a self-join with one parent on both edges.
+template <typename LeftDIA, typename RightDIA, typename JoinFunction>
+auto InnerJoin(const LeftDIA& left, const RightDIA& right, const KeyFirst& /* key_extractor1 */,
+               const KeyFirst& /* key_extractor2 */, const JoinFunction& join_function) {
+    using LeftType = typename LeftDIA::ValueType;
+    using RightType = typename RightDIA::ValueType;
+    static_assert(JoinDesc<JoinFunction>::supported,
+                  "thrill_gpu::InnerJoin: the join function has no GPU descriptor (JoinKeyValues or JoinValues); "
+                  "use the stock api::InnerJoin(left, right, key1, key2, join_fn)");
+    static_assert(std::is_same<typename LeftType::first_type, uint64_t>::value &&
+                  std::is_same<typename RightType::first_type, uint64_t>::value &&
+                  sizeof(typename LeftType::second_type) == 8 && sizeof(typename RightType::second_type) == 8 &&
+                  std::is_trivially_copyable<typename LeftType::second_type>::value &&
+                  std::is_trivially_copyable<typename RightType::second_type>::value,
+                  "thrill_gpu::InnerJoin: both DIAs must hold pair<uint64_t, 8-byte value>; "
+                  "use the stock api::InnerJoin(left, right, key1, key2, join_fn)");
+    using ValueType = decltype(join_function(std::declval<LeftType>(), std::declval<RightType>()));
+    left.AssertValid();
+    right.AssertValid();
+    auto node = tlx::make_counting<GpuJoinNode<ValueType, LeftType, RightType, JoinDesc<JoinFunction>::out_bytes> >(
+        left, right, tg_join_desc { 16, JoinDesc<JoinFunction>::fn });
     return DIA<ValueType>(node);
 }
 
