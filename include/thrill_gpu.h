@@ -16,8 +16,8 @@
  * Device buffers passed in must be 16-byte aligned.  There is NO CPU fallback anywhere behind this ABI.
  *
  * Limits (TG_ERR_TOO_LARGE, checked before any work): every entry point that takes a device item count (tg_radix_sort_local,
- * tg_classify_scatter, tg_hash_aggregate, tg_hash_partition, tg_sort, tg_reduce_by_key, tg_reduce_to_index and their
- * _file / _dev forms) takes at most 2^30 - 1 items per call and worker (n_local), and a worker receives at most 2^30 - 1
+ * tg_classify_scatter, tg_sort_select (per shard), tg_hash_aggregate, tg_hash_partition, tg_range_partition, tg_sort, tg_reduce_by_key,
+ * tg_reduce_to_index and their _file / _dev forms) takes at most 2^30 - 1 items per call and worker (n_local), and a worker receives at most 2^30 - 1
  * items in an exchange: the partition passes count in 30-bit fields.  ReduceToIndex gives each worker fewer than 2^31
  * indices of the result.  Merge (tg_merge and its forms) takes at most 2^30 - 1 items in a worker's k inputs together, and gives
  * each worker at most 2^30 - 1 items of the result; it merges 2..16 inputs of 8- or 16-byte items.  InnerJoin (tg_inner_join
@@ -181,6 +181,19 @@ int tg_classify_scatter(tg_ctx* ctx, const tg_key_desc* desc, const void* d_in, 
                         uint64_t global_index_base, const void* splitters_host, uint32_t p,
                         void* d_out, uint64_t* out_counts);
 
+/* The classification of the multi-worker Sort for p simulated workers on one device (2 <= p <= 16, any ctx): shard w (n_shards[w]
+ * items at d_shards[w], global indices after those of the shards before it) is worker w.  It runs the operator's device code
+ * except the all-gather: worker w draws its sample with the operator's seed into the slot the all-gather fills, the splitters and
+ * their top-byte lookup table are selected on the device as worker w does, and the classification pass of the exchange stores
+ * shard w's items grouped by destination (stable) into d_out[w] instead of the peers' windows.  Writes out_splitters: (p-1) x
+ * (item_bytes + 8) packed as by tg_select_splitters (the sampled item, its global index; zeros when there are no items at all),
+ * out_counts[src * p + dst], and if out_merge_bounds is not NULL, the bucket boundaries the merge pipeline (TG_SORT_PIPELINE=merge)
+ * computes on the stable sort of each shard: out_merge_bounds[w * (p-1) + j].  Shards are read, never modified.  8- or 16-byte
+ * items with any descriptor tg_sort takes for them (records are classified as 16-byte BYTES_BE tuples); otherwise TG_ERR_ARG;
+ * a shard of 2^30 or more items is TG_ERR_TOO_LARGE. */
+int tg_sort_select(tg_ctx* ctx, const tg_key_desc* desc, const void* const* d_shards, const size_t* n_shards, uint32_t p,
+                   uint64_t rng_seed, void* out_splitters, void* const* d_out, uint64_t* out_counts, uint64_t* out_merge_bounds);
+
 /* k-way merge of sorted runs laid back to back in d_runs (run r has run_items[r] items).  Replaces
  * core::MultiwayMergeTree::Next over tlx::LoserTree (core/multiway_merge.hpp:30-116,
  * extlib/tlx/tlx/container/loser_tree.hpp:54-292) as driven by SortNode::PushData (api/sort.hpp:216-271).
@@ -203,6 +216,13 @@ int tg_hash_aggregate(tg_ctx* ctx, const tg_kv_desc* desc, const void* d_in, siz
  * writer_[partition_id] (core/reduce_pre_phase.hpp:57-61). */
 int tg_hash_partition(tg_ctx* ctx, const tg_kv_desc* desc, const void* d_in, size_t n, uint32_t p,
                       void* d_out, uint64_t* out_counts);
+
+/* Range partition of ReduceToIndex (what its exchange classifies by): destination of a 16-byte item with u64 index k is
+ * k < size ? k * p / size : p - 1 (core/reduce_functional.hpp:112-125; worker d's range starts at ceil(d * size / p)).  Stable:
+ * d_out receives the items grouped by destination in input order, out_counts[p] (host) the counts.  1 <= p <= 256; a size with
+ * (size - 1) * p >= 2^64 is TG_ERR_ARG. */
+int tg_range_partition(tg_ctx* ctx, const void* d_in, size_t n, uint64_t size, uint32_t p,
+                       void* d_out, uint64_t* out_counts);
 
 /* The arithmetic of one exchange, pure host code (what every rank derives from the all-gathered p x p count matrix; exported so
  * that the N > 1 host logic is testable without GPUs): counts[src * p + dst] = items rank src holds for rank dst.  For rank `me`:

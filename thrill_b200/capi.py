@@ -96,9 +96,11 @@ SYMBOLS = [
     ("tg_select_splitters", _i, [_P(KeyDesc), _vp, _u64, _u32, _vp]),
     ("tg_draw_samples", _i, [_vp, _P(KeyDesc), _vp, _sz, _u64, _u64, _vp, _P(_u64)]),
     ("tg_classify_scatter", _i, [_vp, _P(KeyDesc), _vp, _sz, _u64, _vp, _u32, _vp, _P(_u64)]),
+    ("tg_sort_select", _i, [_vp, _P(KeyDesc), _P(_vp), _P(_sz), _u32, _u64, _vp, _P(_vp), _P(_u64), _P(_u64)]),
     ("tg_kway_merge", _i, [_vp, _P(KeyDesc), _vp, _P(_u64), _u32, _vp, _vp]),
     ("tg_hash_aggregate", _i, [_vp, _P(KVDesc), _vp, _sz, _vp, _P(_u64)]),
     ("tg_hash_partition", _i, [_vp, _P(KVDesc), _vp, _sz, _u32, _vp, _P(_u64)]),
+    ("tg_range_partition", _i, [_vp, _vp, _sz, _u64, _u32, _vp, _P(_u64)]),
     ("tg_exchange_plan", _i, [_u32, _u32, _P(_u32), _P(_u64), _P(_u64), _P(_u64), _P(_u64), _P(_u64)]),
     ("tg_sort", _i, [_vp, _P(KeyDesc), _vp, _sz, _u64, _P(_vp), _P(_sz)]),
     ("tg_reduce_by_key", _i, [_vp, _P(KVDesc), _vp, _sz, _P(_vp), _P(_sz)]),

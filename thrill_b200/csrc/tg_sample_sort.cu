@@ -257,19 +257,32 @@ bool classify_first() {
     return v != 0;
 }
 
-// samples of every worker and the splitters, all on the device (no host round trip): d_spl[p-1] in LessSampleIndex order,
-// d_ctl = { this worker's global index base, total items, total samples, status flags }.  `items` are WORDS-word items whose
-// canonical key is described by kv.  Collective (one ncclAllGather).
-template <int WORDS>
-int device_splitters(tg_ctx* ctx, const KeyView& kv, const void* d_items, size_t n_local, uint64_t rng_seed, bool too_large,
-                     CanonIdx** d_spl_out, u64** d_ctl_out, unsigned char** d_lut_out = nullptr) {
-    typedef typename ItemT<WORDS>::type Item;
-    const int p = ctx->nranks, me = ctx->rank;
-    unsigned char* d_samp;      // [p] gathered slots | my slot | splitters | ctl
+// The sample workspace of p workers (WS_SAMPLES): [p] gathered slots | this worker's slot | splitters | ctl | LUT.
+// ctl = { this worker's global index base, total items, total samples, status flags }.
+struct SampleWs {
+    unsigned char* slots;
+    unsigned char* mine;
+    CanonIdx* spl;
+    u64* ctl;
+    unsigned char* lut;
+};
+int sample_workspace(tg_ctx* ctx, int p, SampleWs* ws) {
+    unsigned char* d_samp;
     TG_TRY(tg_ws_get(ctx, WS_SAMPLES, (size_t)(p + 1) * SAMPLE_SLOT_BYTES + 8192, (void**)&d_samp));
-    unsigned char* d_mine = d_samp + (size_t)p * SAMPLE_SLOT_BYTES;
-    CanonIdx* d_spl = reinterpret_cast<CanonIdx*>(d_mine + SAMPLE_SLOT_BYTES);
-    u64* d_ctl = reinterpret_cast<u64*>(d_spl + TG_MAX_RANKS);
+    ws->slots = d_samp;
+    ws->mine = d_samp + (size_t)p * SAMPLE_SLOT_BYTES;
+    ws->spl = reinterpret_cast<CanonIdx*>(ws->mine + SAMPLE_SLOT_BYTES);
+    ws->ctl = reinterpret_cast<u64*>(ws->spl + TG_MAX_RANKS);
+    ws->lut = reinterpret_cast<unsigned char*>(ws->ctl + 8);
+    return TG_OK;
+}
+
+// the sample slot of worker `me` at d_slot: its header and its sample in LessSampleIndex order, drawn with the operator's seed.
+// `items` are WORDS-word items whose canonical key is described by kv; too_large: an empty slot that reports the limit.
+template <int WORDS>
+int draw_sample_slot(tg_ctx* ctx, const KeyView& kv, const void* d_items, size_t n_local, uint64_t rng_seed, int me, bool too_large,
+                     unsigned char* d_slot) {
+    typedef typename ItemT<WORDS>::type Item;
     const u64 n_eff = too_large ? 0 : n_local;
     const u64 want = n_eff ? tg_sample_size(n_eff) : 0;
     const u32 ns = (u32)(want < n_eff ? want : n_eff);
@@ -282,20 +295,52 @@ int device_splitters(tg_ctx* ctx, const KeyView& kv, const void* d_items, size_t
         }
         const int grid = (int)((ns + 31) / 32) < ctx->sm_count ? (int)((ns + 31) / 32) : ctx->sm_count;
         TG_LAUNCH(ctx, kern, grid, SRANK_THREADS, smem, (const Item*)d_items, (u64)n_eff,
-                  rng_seed * 0x9E3779B97F4A7C15ull + (u64)me * 0x100000000ull, ns, kv, d_mine);
+                  rng_seed * 0x9E3779B97F4A7C15ull + (u64)me * 0x100000000ull, ns, kv, d_slot);
     }
     else {
         SampleHdr* h = (SampleHdr*)((u64*)ctx->pinned + 2560);        // (pinned scratch, byte offset 20 KB)
         *h = SampleHdr{ 0, 0, too_large ? 1ull : 0ull, 0 };
-        TG_CUDA(ctx, cudaMemcpyAsync(d_mine, h, sizeof(SampleHdr), cudaMemcpyHostToDevice, ctx->stream));
+        TG_CUDA(ctx, cudaMemcpyAsync(d_slot, h, sizeof(SampleHdr), cudaMemcpyHostToDevice, ctx->stream));
     }
-    TG_NCCL(ctx, ncclAllGather(d_mine, d_samp, SAMPLE_SLOT_BYTES, ncclUint8, ctx->comm, ctx->stream));
-    TG_LAUNCH(ctx, select_splitters_kernel, (p * SAMPLE_MAX + 255) / 256, 256, 0, (const unsigned char*)d_samp, p, me, d_spl, d_ctl);
-    unsigned char* d_lut = reinterpret_cast<unsigned char*>(d_ctl + 8);
-    TG_LAUNCH(ctx, splitter_lut_kernel, 1, 256, 0, (const CanonIdx*)d_spl, (u32)(p - 1), kv, d_lut);
-    if (d_lut_out) *d_lut_out = d_lut;
-    *d_spl_out = d_spl;
-    *d_ctl_out = d_ctl;
+    return TG_OK;
+}
+
+// splitters, ctl and LUT of worker `me` from the p gathered slots (every worker computes the same splitters; ctl[0] is its own)
+int splitters_from_slots(tg_ctx* ctx, const KeyView& kv, const SampleWs& ws, int p, int me) {
+    TG_LAUNCH(ctx, select_splitters_kernel, (p * SAMPLE_MAX + 255) / 256, 256, 0, (const unsigned char*)ws.slots, p, me, ws.spl, ws.ctl);
+    TG_LAUNCH(ctx, splitter_lut_kernel, 1, 256, 0, (const CanonIdx*)ws.spl, (u32)(p - 1), kv, ws.lut);
+    return TG_OK;
+}
+
+// samples of every worker and the splitters, all on the device (no host round trip): d_spl[p-1] in LessSampleIndex order,
+// d_ctl as in SampleWs.  Collective (one ncclAllGather).
+template <int WORDS>
+int device_splitters(tg_ctx* ctx, const KeyView& kv, const void* d_items, size_t n_local, uint64_t rng_seed, bool too_large,
+                     CanonIdx** d_spl_out, u64** d_ctl_out, unsigned char** d_lut_out = nullptr) {
+    const int p = ctx->nranks, me = ctx->rank;
+    SampleWs ws;
+    TG_TRY(sample_workspace(ctx, p, &ws));
+    TG_TRY(draw_sample_slot<WORDS>(ctx, kv, d_items, n_local, rng_seed, me, too_large, ws.mine));
+    TG_NCCL(ctx, ncclAllGather(ws.mine, ws.slots, SAMPLE_SLOT_BYTES, ncclUint8, ctx->comm, ctx->stream));
+    TG_TRY(splitters_from_slots(ctx, kv, ws, p, me));
+    if (d_lut_out) *d_lut_out = ws.lut;
+    *d_spl_out = ws.spl;
+    *d_ctl_out = ws.ctl;
+    return TG_OK;
+}
+
+// The merge pipeline's bucket boundaries of one shard: the per-splitter tie counts on the unsorted shard (item i has global
+// index gbase + i), the stable local sort (d_in or d_tmp ends up holding it: *d_sorted), then bnd[j] = lower_bound(sorted,
+// splitter j's key) + tie[j].  d_tie: 4 KiB of device scratch.
+template <int WORDS>
+int shard_boundaries(tg_ctx* ctx, const tg_key_desc* desc, const KeyView& kv, void* d_in, void* d_tmp, size_t n_local, u64 gbase,
+                     const CanonIdx* d_spl, u32 nspl, u32* d_tie, u64* d_bnd, void** d_sorted) {
+    typedef typename ItemT<WORDS>::type Item;
+    TG_CUDA(ctx, cudaMemsetAsync(d_tie, 0, 4096, ctx->stream));
+    if (n_local && nspl)
+        TG_LAUNCH(ctx, tie_count_kernel<WORDS>, ctx->sm_count * 4, 512, 0, (const Item*)d_in, (u32)n_local, gbase, kv, d_spl, nspl, d_tie);
+    TG_TRY(tg_radix_sort_items(ctx, desc, d_in, d_tmp, n_local, d_sorted));
+    if (nspl) TG_LAUNCH(ctx, boundaries_kernel<WORDS>, (nspl + 63) / 64, 64, 0, (const Item*)*d_sorted, (u32)n_local, kv, d_spl, nspl, d_tie, d_bnd);
     return TG_OK;
 }
 
@@ -374,14 +419,10 @@ int sort_multi_impl(tg_ctx* ctx, const tg_key_desc* desc, const KeyView& kv, voi
     // (3) per-splitter tie counts on the unsorted shard, (4) local radix sort, (5) bucket boundaries
     u32* d_tie = (u32*)(d_ctl + 1024);
     u64* d_bnd = d_ctl + 2048;
-    TG_CUDA(ctx, cudaMemsetAsync(d_tie, 0, 4096, ctx->stream));
-    if (n_local && nspl)
-        TG_LAUNCH(ctx, tie_count_kernel<WORDS>, ctx->sm_count * 4, 512, 0, (const Item*)d_in, (u32)n_local, prefix, kv, d_spl, nspl, d_tie);
     void* d_tmp;
     TG_TRY(tg_ws_get(ctx, WS_SORT_TMP, n_local * s, &d_tmp));
     void* d_sorted;      // d_in or d_tmp, whichever the last pass wrote
-    TG_TRY(tg_radix_sort_items(ctx, desc, d_in, d_tmp, n_local, &d_sorted));
-    if (nspl) TG_LAUNCH(ctx, boundaries_kernel<WORDS>, (nspl + 63) / 64, 64, 0, (const Item*)d_sorted, (u32)n_local, kv, d_spl, nspl, d_tie, d_bnd);
+    TG_TRY(shard_boundaries<WORDS>(ctx, desc, kv, d_in, d_tmp, n_local, prefix, d_spl, nspl, d_tie, d_bnd, &d_sorted));
     TG_CUDA(ctx, cudaMemcpyAsync(h, d_bnd, 8 * nspl, cudaMemcpyDeviceToHost, ctx->stream));
     TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     std::vector<u64> send_cnt(p), send_off(p + 1, 0);
@@ -428,6 +469,73 @@ int sort_multi_impl(tg_ctx* ctx, const tg_key_desc* desc, const KeyView& kv, voi
     return TG_OK;
 }
 
+
+// tg_sort_select: the operator's non-collective steps for p simulated workers on one device.  Worker w's sample slot is drawn
+// where the all-gather would put it; then, worker by worker, the splitters with me = w (its global index base lands in ctl[0])
+// and the classification pass that the P2P exchange runs, storing locally.
+template <int WORDS>
+int sort_select_impl(tg_ctx* ctx, const tg_key_desc* desc, const KeyView& kv, const void* const* d_shards, const size_t* n_shards,
+                     int p, uint64_t rng_seed, void* out_splitters, void* const* d_out, uint64_t* out_counts, uint64_t* out_merge_bounds) {
+    typedef typename ItemT<WORDS>::type Item;
+    const size_t s = sizeof(Item);
+    const u32 nspl = (u32)(p - 1);
+    SampleWs ws;
+    TG_TRY(sample_workspace(ctx, p, &ws));
+    u64 prefix[TG_MAX_RANKS + 1] = { 0 };
+    // (the header of an empty shard is staged in the same pinned words for every worker: the bytes are the same each time)
+    for (int w = 0; w < p; ++w) {
+        prefix[w + 1] = prefix[w] + n_shards[w];
+        TG_TRY(draw_sample_slot<WORDS>(ctx, kv, d_shards[w], n_shards[w], rng_seed, w, false, ws.slots + (size_t)w * SAMPLE_SLOT_BYTES));
+    }
+    u64* h = (u64*)ctx->pinned + 3072;               // byte offset 24 KB: splitters | counts | bounds | splitter items
+    CanonIdx* h_spl = (CanonIdx*)h;
+    u32* h_cnt = (u32*)(h_spl + TG_MAX_RANKS);
+    u64* h_bnd = (u64*)(h_cnt + RADIX);
+    for (int w = 0; w < p; ++w) {
+        TG_TRY(splitters_from_slots(ctx, kv, ws, p, w));
+        SplitterDigit fn = { ws.spl, nspl, 0, kv, ws.ctl, ws.lut, nullptr, nullptr };
+        u32* d_tot = nullptr;
+        TG_TRY((partition_chunked<WORDS, SplitterDigit>(ctx, d_shards[w], d_out[w], n_shards[w], fn, &d_tot, nullptr)));
+        TG_CUDA(ctx, cudaMemcpyAsync(h_cnt, d_tot, (size_t)p * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        if (w == 0) TG_CUDA(ctx, cudaMemcpyAsync(h_spl, ws.spl, nspl * sizeof(CanonIdx), cudaMemcpyDeviceToHost, ctx->stream));
+        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        for (int d = 0; d < p; ++d) out_counts[(size_t)w * p + d] = h_cnt[d];
+    }
+    // the splitters as tg_select_splitters packs them: the sampled item, then its global index (no items: no sample, zeros)
+    unsigned char* o = (unsigned char*)out_splitters;
+    unsigned char* h_item = (unsigned char*)(h_bnd + TG_MAX_RANKS);
+    memset(o, 0, nspl * (s + 8));
+    if (prefix[p]) {
+        for (u32 j = 0; j < nspl; ++j) {
+            const u64 g = h_spl[j].idx;
+            memset(h_item + j * s, 0, s);
+            if (g >= prefix[p]) continue;                // (not a sampled position: reported as is, with a zero item)
+            int w = 0;
+            while (g >= prefix[w + 1]) ++w;
+            TG_CUDA(ctx, cudaMemcpyAsync(h_item + j * s, (const char*)d_shards[w] + (g - prefix[w]) * s, s, cudaMemcpyDeviceToHost, ctx->stream));
+        }
+        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        for (u32 j = 0; j < nspl; ++j) {
+            memcpy(o + j * (s + 8), h_item + j * s, s);
+            memcpy(o + j * (s + 8) + s, &h_spl[j].idx, 8);
+        }
+    }
+    if (!out_merge_bounds) return TG_OK;
+    u64* d_misc;
+    TG_TRY(tg_ws_get(ctx, WS_MISC, 1 << 16, (void**)&d_misc));
+    for (int w = 0; w < p; ++w) {
+        const size_t n = n_shards[w];
+        void *d_copy, *d_tmp, *d_sorted;
+        TG_TRY(tg_ws_get(ctx, WS_AUX, (n + 1) * s, &d_copy));
+        TG_TRY(tg_ws_get(ctx, WS_SORT_TMP, (n + 1) * s, &d_tmp));
+        if (n) TG_CUDA(ctx, cudaMemcpyAsync(d_copy, d_shards[w], n * s, cudaMemcpyDeviceToDevice, ctx->stream));
+        TG_TRY(shard_boundaries<WORDS>(ctx, desc, kv, d_copy, d_tmp, n, prefix[w], ws.spl, nspl, (u32*)(d_misc + 1024), d_misc + 2048, &d_sorted));
+        TG_CUDA(ctx, cudaMemcpyAsync(h_bnd, d_misc + 2048, nspl * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        for (u32 j = 0; j < nspl; ++j) out_merge_bounds[(size_t)w * nspl + j] = h_bnd[j];
+    }
+    return TG_OK;
+}
 
 // ---- records with payload (TeraSort: Record{uint8 key[10]; uint8 value[90]}, examples/terasort/terasort.cpp:31-42) ----
 // Sorted through 16-byte tuples {key bytes (<= 12, zero padded), u32 position}: build (reads only the sectors that hold the
@@ -718,6 +826,23 @@ int tg_classify_scatter(tg_ctx* ctx, const tg_key_desc* desc, const void* d_in, 
     TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     for (uint32_t r = 0; r < p; ++r) out_counts[r] = hc[r];
     return TG_OK;
+}
+
+int tg_sort_select(tg_ctx* ctx, const tg_key_desc* desc, const void* const* d_shards, const size_t* n_shards, uint32_t p,
+                   uint64_t rng_seed, void* out_splitters, void* const* d_out, uint64_t* out_counts, uint64_t* out_merge_bounds) {
+    KeyView kv;
+    if (!ctx || make_key_view(desc, &kv) != TG_OK || (desc->item_bytes != 8 && desc->item_bytes != 16))
+        return tg_set_error(ctx, TG_ERR_ARG, "sort_select: unsupported descriptor (8- or 16-byte items)");
+    if (p < 2 || p > TG_MAX_RANKS || !d_shards || !n_shards || !out_splitters || !d_out || !out_counts)
+        return tg_set_error(ctx, TG_ERR_ARG, "sort_select: p=%u or a NULL argument", p);
+    for (uint32_t w = 0; w < p; ++w)
+        if (n_shards[w] && (!d_shards[w] || !d_out[w])) return tg_set_error(ctx, TG_ERR_ARG, "sort_select: shard %u is NULL", w);
+    for (uint32_t w = 0; w < p; ++w)
+        if (n_shards[w] >= (1u << 30)) return tg_set_error(ctx, TG_ERR_TOO_LARGE, "sort_select: shard %u has %zu items", w, n_shards[w]);
+    TG_CUDA(ctx, cudaSetDevice(ctx->device));
+    return desc->item_bytes == 8
+               ? sort_select_impl<1>(ctx, desc, kv, d_shards, n_shards, (int)p, rng_seed, out_splitters, d_out, out_counts, out_merge_bounds)
+               : sort_select_impl<2>(ctx, desc, kv, d_shards, n_shards, (int)p, rng_seed, out_splitters, d_out, out_counts, out_merge_bounds);
 }
 
 int tg_sort(tg_ctx* ctx, const tg_key_desc* desc, void* d_in, size_t n_local, uint64_t rng_seed, void** out_dptr, size_t* out_n) {
