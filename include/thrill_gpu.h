@@ -22,7 +22,9 @@
  * indices of the result.  Merge (tg_merge and its forms) takes at most 2^30 - 1 items in a worker's k inputs together, and gives
  * each worker at most 2^30 - 1 items of the result; it merges 2..16 inputs of 8- or 16-byte items.  InnerJoin (tg_inner_join
  * and its _file form) takes at most 2^30 - 1 items per worker and side, before and after its exchange, and gives each worker at
- * most 2^30 - 1 items of the result.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
+ * most 2^30 - 1 items of the result.  GroupByKey and GroupToIndex (tg_group_by_key, tg_group_to_index and their _file forms)
+ * take at most 2^30 - 1 items per worker, before and after their exchange, and tg_mod_partition at most 2^30 - 1 items per call.
+ * The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
  ******************************************************************************/
 #ifndef THRILL_GPU_H
 #define THRILL_GPU_H
@@ -360,6 +362,40 @@ int tg_inner_join(tg_ctx* ctx, const tg_join_desc* desc, const void* d_left, siz
  * result is fetched with tg_fetch_output or taken with tg_output_detach (item_bytes 24 or 16) */
 int tg_inner_join_file(tg_ctx* ctx, const tg_join_desc* desc, const tg_merge_input* left, const tg_merge_input* right,
                        size_t* out_items);
+
+/* ---- GroupByKey / GroupToIndex: a DIA<pair<u64, V>> grouped by .first (DIA::GroupByKey, api/group_by_key.hpp:46-428;
+ * DIA::GroupToIndex, api/group_to_index.hpp:36-290) ---------------------------------------------------------------------------
+ * The reference's nodes work in two halves: MainOp exchanges every item to the owner of its key and sorts each worker's share by
+ * the key (group_by_key.hpp:348-376, group_to_index.hpp:234-254); PushData walks the sorted items and calls the user's group
+ * function once per group (group_by_key.hpp:204-331, group_to_index.hpp:116-215).  These entry points replace the first half;
+ * the group function, with its arbitrary output type, stays on the host (GpuGroupNode in thrill_b200/host/).  The result of a
+ * worker is its share of the 16-byte items (uint64_t key, 8-byte value: any type, copied as bits) sorted by the key, and stable:
+ * equal keys keep their global input order (global position = position in the concatenation of the workers' shards).  The
+ * reference sorts with std::sort and leaves that order open; this is one of the orders it allows.
+ * Placement:
+ *   GroupByKey    worker key % p owns a key: hash_function(key) % p (group_by_key.hpp:149-159) with the default hash
+ *                 std::hash<uint64_t>, the identity in libstdc++ (:419-428).  (Not ReduceByKey's Hash128to64.)
+ *   GroupToIndex  worker k * p / result_size owns index k (CalculatePartition, group_to_index.hpp:98-105): worker r answers for
+ *                 [*out_begin, *out_end) = Range(0, result_size).Partition(r, p) = [ceil(r * size / p), ceil((r+1) * size / p)),
+ *                 ReduceToIndex's ranges.  An index >= result_size (an assert in the reference) is TG_ERR_ARG on every rank: such
+ *                 items go to the last worker, whose verdict an all-reduce hands to the others.  A result_size with
+ *                 (result_size - 1) * p >= 2^64 is TG_ERR_ARG.
+ * The input is read, never modified; 2^30 or more items on a worker, before or after the exchange, is TG_ERR_TOO_LARGE on every
+ * rank (the exchange's count matrix decides it).  Host round trips: GroupByKey none with p = 1, one with p > 1 (the count matrix);
+ * GroupToIndex one with p = 1 (the index check), two with p > 1 (the count matrix and the all-reduce of the index check).
+ * Collective. */
+/* on device buffers; *out_dptr as for tg_sort (ctx-owned, valid until the next operator call) */
+int tg_group_by_key(tg_ctx* ctx, const void* d_in, size_t n_local, void** out_dptr, size_t* out_n);
+int tg_group_to_index(tg_ctx* ctx, const void* d_in, size_t n_local, uint64_t result_size, void** out_dptr, size_t* out_n,
+                      uint64_t* out_begin, uint64_t* out_end);
+/* the drop-in calls (GpuGroupNode::Execute): the input is a host File (Blocks) or a device File (read in place, left intact); the
+ * result (16-byte items) is fetched with tg_fetch_output or taken with tg_output_detach */
+int tg_group_by_key_file(tg_ctx* ctx, const tg_merge_input* in, size_t* out_items);
+int tg_group_to_index_file(tg_ctx* ctx, const tg_merge_input* in, uint64_t result_size, size_t* out_items,
+                           uint64_t* out_begin, uint64_t* out_end);
+/* kernel level (tests of the placement on one GPU): GroupByKey's partition, destination of a 16-byte item = key % p.  Stable:
+ * d_out receives the items grouped by destination in input order, out_counts[p] (host) the counts.  1 <= p <= 256. */
+int tg_mod_partition(tg_ctx* ctx, const void* d_in, size_t n, uint32_t p, void* d_out, uint64_t* out_counts);
 
 /* ---- synthetic inputs of SURVEY.md §8(d), generated on the device (bench / tests support) ------------ */
 int tg_gen_sort_uniform(tg_ctx* ctx, void* d_out, uint64_t begin, uint64_t n, uint64_t seed);

@@ -7,6 +7,7 @@ Mirrors (same names, argument meaning and error behaviour) the slice of thrill/a
     DIA<T>::ReducePair(reduce_fn)          thrill/api/reduce_by_key.hpp:410-449
     DIA<T>::ReduceByKey(key_ex, reduce_fn) thrill/api/reduce_by_key.hpp:312-363
     DIA<T>::Merge(second, cmp) / api::Merge thrill/api/merge.hpp:674-721
+    DIA<T>::GroupByKey / GroupToIndex      thrill/api/group_by_key.hpp:419-428, group_to_index.hpp:257-290
     api::InnerJoin(l, r, key1, key2, fn)   thrill/api/inner_join.hpp:700-827
     DIA<T>::Size / AllGather / Gather      thrill/api/size.hpp, all_gather.hpp, gather.hpp
 A DIA here holds its local shard as a host numpy array — the stand-in for a data::File whose Blocks are
@@ -202,6 +203,34 @@ def InnerJoin(first, second, key_extractor1, key_extractor2, join_function, **kw
     return DIA(first.ctx, first._fetch(n_out.value, dtype, dtype.itemsize, kw.get("_pinned_out")))
 
 
+class GroupIterator(object):
+    """the iterator handed to a group function (api::GroupByIterator, api/group_by_iterator.hpp:47-127): HasNext() / Next() over
+    one group of the key-sorted items; Next() gives a (key, value) tuple of ints"""
+
+    def __init__(self, items):
+        self._keys, self._vals = items["key"], items["val"]
+        self._pos, self._equal = 0, True
+        self._key = int(self._keys[0])
+
+    def HasNext(self):
+        return self._pos < len(self._keys) and self._equal
+
+    def Next(self):
+        k, v = int(self._keys[self._pos]), int(self._vals[self._pos])
+        self._pos += 1
+        if self._pos < len(self._keys) and int(self._keys[self._pos]) != self._key:
+            self._key = int(self._keys[self._pos])
+            self._equal = False
+        return k, v
+
+    def _has_next_for_real(self):
+        return self._pos < len(self._keys)
+
+    def _get_next_key(self):
+        self._equal = True
+        return self._key
+
+
 class DIA(object):
     def __init__(self, ctx, items):
         self.ctx = ctx
@@ -296,6 +325,55 @@ class DIA(object):
         out = DIA(self.ctx, self._fetch(n_out.value, KV, 16, _pinned_out))
         out.index_begin = int(begin.value)
         return out
+
+    # ---- DIA<T>::GroupByKey / GroupToIndex (api/group_by_key.hpp:419-428, api/group_to_index.hpp:257-290) -------------------
+    def _group(self, what, key_extractor, size=None):
+        if key_extractor is not KeyIsFirst:
+            raise capi.ThrillGpuError("%s: only the pair.first key extractor is recognised by the GPU path" % what)
+        if not (self.items.ndim == 1 and self.items.dtype == KV):
+            raise capi.ThrillGpuError("%s: items must be pair<uint64_t, 8-byte value>" % what)
+        blocks, nb = self._blocks(self.items)
+        inp = capi.MergeInput(None, C.cast(blocks, C.POINTER(capi.Block)), nb)
+        n_out, begin, end = C.c_size_t(), C.c_uint64(), C.c_uint64()
+        tg = self.ctx.tg
+        if size is None:
+            tg.ck(tg.L.tg_group_by_key_file(tg.h, C.byref(inp), C.byref(n_out)))
+        else:
+            tg.ck(tg.L.tg_group_to_index_file(tg.h, C.byref(inp), int(size), C.byref(n_out), C.byref(begin), C.byref(end)))
+        return self._fetch(n_out.value, KV, 16), int(begin.value), int(end.value)
+
+    def GroupByKey(self, key_extractor, group_function, dtype):
+        """items: pair<uint64_t, 8-byte value>; group_function(iterator, key) is called once per group of this worker's share
+        (worker key % p owns a key) in ascending key order, with an iterator that has HasNext() and Next() over the group's
+        items in global input order; a function that stops early is called again with the rest of its group.  The result
+        holds what it returns, as an array of `dtype`."""
+        grouped, _, _ = self._group("GroupByKey", key_extractor)
+        out = []
+        if len(grouped):
+            it = GroupIterator(grouped)
+            while it._has_next_for_real():
+                out.append(group_function(it, it._get_next_key()))
+        return DIA(self.ctx, np.array(out, dtype=dtype))
+
+    def GroupToIndex(self, key_extractor, group_function, size, neutral_element, dtype):
+        """items: pair<uint64_t index, 8-byte value>; one result per index of this worker's range
+        Range(0, size).Partition(rank, p): group_function(iterator, index) where the index has items, neutral_element where it
+        has none.  An index >= size raises.  .index_begin = first index of the range."""
+        grouped, begin, end = self._group("GroupToIndex", key_extractor, size)
+        out = []
+        curr = begin
+        if len(grouped):
+            it = GroupIterator(grouped)
+            while it._has_next_for_real():
+                if it._get_next_key() != curr:
+                    out.append(neutral_element)
+                else:
+                    out.append(group_function(it, it._get_next_key()))
+                curr += 1
+        out.extend([neutral_element] * (end - curr))
+        res = DIA(self.ctx, np.array(out, dtype=dtype))
+        res.index_begin = begin
+        return res
 
     def ReduceByKey(self, key_extractor, reduce_function):
         if key_extractor is not KeyIsFirst:

@@ -121,6 +121,11 @@ SYMBOLS = [
     ("tg_merge_plan", _i, [_u32, _u32, _P(_u64), _P(_u64), _P(_u64), _P(_u64)]),
     ("tg_inner_join", _i, [_vp, _P(JoinDesc), _vp, _sz, _vp, _sz, _P(_vp), _P(_sz)]),
     ("tg_inner_join_file", _i, [_vp, _P(JoinDesc), _P(MergeInput), _P(MergeInput), _P(_sz)]),
+    ("tg_group_by_key", _i, [_vp, _vp, _sz, _P(_vp), _P(_sz)]),
+    ("tg_group_to_index", _i, [_vp, _vp, _sz, _u64, _P(_vp), _P(_sz), _P(_u64), _P(_u64)]),
+    ("tg_group_by_key_file", _i, [_vp, _P(MergeInput), _P(_sz)]),
+    ("tg_group_to_index_file", _i, [_vp, _P(MergeInput), _u64, _P(_sz), _P(_u64), _P(_u64)]),
+    ("tg_mod_partition", _i, [_vp, _vp, _sz, _u32, _vp, _P(_u64)]),
     ("tg_transfer_bytes", _i, [_vp, _P(_u64), _P(_u64)]),
     ("tg_gen_sort_uniform", _i, [_vp, _vp, _u64, _u64, _u64]),
     ("tg_gen_reduce_uniform", _i, [_vp, _vp, _u64, _u64, _u64, _u64, _i]),

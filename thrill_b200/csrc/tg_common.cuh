@@ -70,7 +70,8 @@ enum { WS_SORT_TMP = 0, WS_SORT_STATUS = 1, WS_SORT_HIST = 2, WS_XCHG_SEND = 3, 
        WS_MISC = 5, WS_TABLE = 6, WS_OUT = 7, WS_IN = 8, WS_AUX = 9, WS_AUX2 = 10, WS_SAMPLES = 11,
        WS_SEG_TILES = 12, WS_SEG_TABLES = 13, WS_SORT_STATUS2 = 14,
        WS_SORT_HIST2 = 15, WS_SEG_TILES2 = 16, WS_DENSE = 17, WS_XCTL = 18, WS_REC = 19, WS_HOT = 20,
-       // InnerJoin (tg_join.cu): the sorted sides (items + sort scratch each), counts / offsets / splits, the output
+       // InnerJoin (tg_join.cu): the sorted sides (items + sort scratch each), counts / offsets / splits, the output.
+       // GroupByKey / GroupToIndex (tg_group.cu) sort into WS_JOIN_L: their result is the sorted items
        WS_JOIN_L = 21, WS_JOIN_R = 22, WS_JOIN_AUX = 23, WS_JOIN_OUT = 24 };
 
 int tg_set_error(tg_ctx* ctx, int status, const char* fmt, ...);

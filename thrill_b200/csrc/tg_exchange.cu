@@ -5,6 +5,8 @@
 
 #include "tg_exchange.cuh"
 
+int tg_radix_sort_items(tg_ctx* ctx, const tg_key_desc* desc, void* d_items, void* d_tmp, size_t n, void** result);
+
 namespace tgp {
 
 namespace {
@@ -211,6 +213,17 @@ int evacuate_window_inputs(tg_ctx* ctx, const void** in, const size_t* bytes, ui
         const char* q = (const char*)in[j];
         if (bytes[j] && q >= lo && q < hi) in[j] = d + (q - lo);
     }
+    return TG_OK;
+}
+
+int sort_pairs_into(tg_ctx* ctx, int slot, const void* src, u64 n, const ulonglong2** sorted) {
+    ulonglong2* buf;
+    TG_TRY(tg_ws_get(ctx, slot, (2 * n + 2) * 16, (void**)&buf));
+    if (n) TG_CUDA(ctx, cudaMemcpyAsync(buf, src, n * 16, cudaMemcpyDeviceToDevice, ctx->stream));
+    const tg_key_desc sd = { 16, 0, 8, TG_KEY_UINT_LE, 0, 1 };
+    void* res = buf;
+    TG_TRY(tg_radix_sort_items(ctx, &sd, buf, buf + n + 1, n, &res));
+    *sorted = (const ulonglong2*)res;
     return TG_OK;
 }
 

@@ -49,6 +49,43 @@ struct HashDigit {
     __device__ __forceinline__ u32 operator()(const ulonglong2& v, u32) const { return (u32)(hash128to64_dev(0, v.x) % p); }
 };
 
+// destination worker of a 16-byte (u64 key, value) item: key % p, the owner of a key in GroupByKey (hash_function(key) % p,
+// api/group_by_key.hpp:149-159, with the default std::hash<uint64_t>, the identity in libstdc++, :419-428).
+// Computed from the two 32-bit halves, key % p = ((hi % p) * (2^32 % p) + lo % p) % p, so that no 64-bit division subroutine
+// (and its register pressure: the partition pass then spills) enters the pass; exact for p <= 2^16 (the partition takes p <= 256).
+struct ModDigit {
+    u32 p;
+    u32 two32_mod_p;                        // 2^32 % p
+    static ModDigit make(u32 p) { return ModDigit{ p, (u32)((1ull << 32) % p) }; }
+    static constexpr bool kStoreDigit = true;
+    static constexpr bool kHasDrop = false;
+    static constexpr int kScratch = 0;
+    __device__ __forceinline__ void init() {}
+    __device__ __forceinline__ u32 operator()(const ulonglong2& v, u32) const {
+        const u32 hi = (u32)(v.x >> 32) % p, lo = (u32)v.x % p;
+        return (hi * two32_mod_p + lo) % p;
+    }
+};
+
+// destination worker of index k: k * p / size (ReduceByIndex / Range::FindPartition, core/reduce_functional.hpp:112-125,
+// common/math.hpp:98-100; CalculatePartition in GroupToIndex, api/group_to_index.hpp:98-105); out-of-range indices are parked
+// on the last worker, which reports them
+struct RangeDigit {
+    u64 size;
+    u32 p;
+    static constexpr bool kStoreDigit = true;
+    static constexpr bool kHasDrop = false;
+    static constexpr int kScratch = 0;
+    __device__ __forceinline__ void init() {}
+    __device__ __forceinline__ u32 operator()(const ulonglong2& v, u32) const {
+        return v.x < size ? (u32)(v.x * p / size) : p - 1;
+    }
+};
+
+// the first index of worker r's range: Range(0, size).Partition(r, p) = ceil(r * size / p) (common/math.hpp:85-94); worker r
+// answers for [range_begin(r), range_begin(r + 1)), the indices RangeDigit sends to it
+inline u64 range_begin(u64 r, u64 size, u64 p) { return (u64)(((unsigned __int128)r * size + p - 1) / p); }
+
 // Stable partition of n local items by fn (destination worker, < p) + Alltoallv.  Collective.
 // n >= 2^30 (over the per-call limit): this rank sends nothing and reports 2^30 items for worker 0 in its counts, so that
 // xchg_counts returns TG_ERR_TOO_LARGE on every rank and none is left waiting in a collective.
@@ -129,6 +166,21 @@ int exchange_scatter(tg_ctx* ctx, const void* d_in, size_t n, const DigitFn& fn,
     TG_NCCL(ctx, ncclGroupEnd());
     if (xprof >= 0) tg_prof_end(ctx, xprof);
     return TG_OK;
+}
+
+// The owner-by-key pipeline of 16-byte (u64 key, value) items (InnerJoin's sides, GroupByKey, GroupToIndex).
+// n items from src into workspace `slot` (items | sort scratch), then the stable local radix sort by the key; *sorted = the
+// result, in the slot.  src is read, never modified.  (tg_exchange.cu)
+int sort_pairs_into(tg_ctx* ctx, int slot, const void* src, u64 n, const ulonglong2** sorted);
+
+// one exchange by fn, then the received items (every worker's, in rank order: stable) sorted in `slot`.  Collective.
+template <class DigitFn>
+int exchange_sort_pairs(tg_ctx* ctx, int slot, const void* d_in, size_t n, const DigitFn& fn, const ulonglong2** sorted,
+                        u64* n_recv) {
+    XchgResult xr;
+    TG_TRY((exchange_scatter<2, DigitFn>(ctx, d_in, n, fn, &xr)));
+    *n_recv = xr.n_recv;
+    return sort_pairs_into(ctx, slot, xr.d_recv, xr.n_recv, sorted);
 }
 
 }  // namespace tgp

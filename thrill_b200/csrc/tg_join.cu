@@ -18,8 +18,6 @@
 #include "tg_keys.cuh"
 #include "tg_exchange.cuh"
 
-int tg_radix_sort_items(tg_ctx* ctx, const tg_key_desc* desc, void* d_items, void* d_tmp, size_t n, void** result);
-
 using namespace tgp;
 
 namespace {
@@ -207,27 +205,6 @@ int check_join_args(tg_ctx* ctx, const tg_join_desc* desc) {
     return TG_OK;
 }
 
-// n items of one side from src into the side's slot (items | sort scratch), then the stable sort by the key; *sorted = the result
-int sort_side(tg_ctx* ctx, int slot, const void* src, u64 n, const Pair** sorted) {
-    Pair* buf;
-    TG_TRY(tg_ws_get(ctx, slot, (2 * n + 2) * 16, (void**)&buf));
-    if (n) TG_CUDA(ctx, cudaMemcpyAsync(buf, src, n * 16, cudaMemcpyDeviceToDevice, ctx->stream));
-    const tg_key_desc sd = { 16, 0, 8, TG_KEY_UINT_LE, 0, 1 };
-    void* res = buf;
-    TG_TRY(tg_radix_sort_items(ctx, &sd, buf, buf + n + 1, n, &res));
-    *sorted = (const Pair*)res;
-    return TG_OK;
-}
-
-// the exchange of one side: its items, received from every worker, end up sorted in `slot`
-int exchange_side(tg_ctx* ctx, int slot, const void* d_in, size_t n, const Pair** sorted, u64* n_recv) {
-    HashDigit fn = { (u32)ctx->nranks };
-    XchgResult xr;
-    TG_TRY((exchange_scatter<2, HashDigit>(ctx, d_in, n, fn, &xr)));
-    *n_recv = xr.n_recv;
-    return sort_side(ctx, slot, xr.d_recv, xr.n_recv, sorted);
-}
-
 int join_impl(tg_ctx* ctx, const tg_join_desc* desc, const void* d_left, size_t n_left, const void* d_right, size_t n_right,
               void** out_dptr, size_t* out_n) {
     const int p = ctx->nranks;
@@ -237,8 +214,8 @@ int join_impl(tg_ctx* ctx, const tg_join_desc* desc, const void* d_left, size_t 
         if (n_left >= JOIN_LIMIT || n_right >= JOIN_LIMIT)
             return tg_set_error(ctx, TG_ERR_TOO_LARGE, "inner_join: %zu x %zu items (limit 2^30 - 1 per side)", n_left, n_right);
         nl = n_left; nr = n_right;
-        TG_TRY(sort_side(ctx, WS_JOIN_L, d_left, nl, &L));
-        TG_TRY(sort_side(ctx, WS_JOIN_R, d_right, nr, &R));
+        TG_TRY(sort_pairs_into(ctx, WS_JOIN_L, d_left, nl, &L));
+        TG_TRY(sort_pairs_into(ctx, WS_JOIN_R, d_right, nr, &R));
     }
     else {
         // (an input inside the exchange window is moved out of the peers' way first; the left side's received items are in
@@ -247,8 +224,9 @@ int join_impl(tg_ctx* ctx, const tg_join_desc* desc, const void* d_left, size_t 
         const size_t bytes[2] = { n_left < JOIN_LIMIT ? n_left * 16 : 0, n_right < JOIN_LIMIT ? n_right * 16 : 0 };
         TG_TRY(xwin_negotiate(ctx));
         TG_TRY(evacuate_window_inputs(ctx, in, bytes, 2));
-        TG_TRY(exchange_side(ctx, WS_JOIN_L, in[0], n_left, &L, &nl));
-        TG_TRY(exchange_side(ctx, WS_JOIN_R, in[1], n_right, &R, &nr));
+        const HashDigit fn = { (u32)p };
+        TG_TRY(exchange_sort_pairs(ctx, WS_JOIN_L, in[0], n_left, fn, &L, &nl));
+        TG_TRY(exchange_sort_pairs(ctx, WS_JOIN_R, in[1], n_right, fn, &R, &nr));
     }
     // scratch: scalars (m, largest m) | packed counts | offsets | tile sums | tile bases | count splits | emit splits
     const u32 nct = (u32)((nl + nr + JC_TILE - 1) / JC_TILE);

@@ -845,21 +845,8 @@ int run_partitioned_aggregate(tg_ctx* ctx, int op, const void* d_in, u64 n, void
     return read_cursor(ctx, sc, out_distinct);
 }
 
-// ---- ReduceToIndex: range partition and the dense result ---------------------------------------------------------------
-// destination worker of index k: k * p / size (ReduceByIndex / Range::FindPartition, core/reduce_functional.hpp:112-125,
-// common/math.hpp:98-100); out-of-range indices are parked on the last worker and reported by the dense scatter
-struct RangeDigit {
-    u64 size;
-    u32 p;
-    static constexpr bool kStoreDigit = true;
-    static constexpr bool kHasDrop = false;
-    static constexpr int kScratch = 0;
-    __device__ __forceinline__ void init() {}
-    __device__ __forceinline__ u32 operator()(const ulonglong2& v, u32) const {
-        return v.x < size ? (u32)(v.x * p / size) : p - 1;
-    }
-};
-
+// ---- ReduceToIndex: the dense result (the range partition is RangeDigit, tg_exchange.cuh; out-of-range indices are reported
+// by the dense scatter) ----------------------------------------------------------------------------------------------------
 __global__ void fill_dense_kernel(ulonglong2* __restrict__ out, u64 n, ulonglong2 neutral) {
     const u64 stride = (u64)gridDim.x * blockDim.x;
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = neutral;
@@ -975,10 +962,9 @@ int tg_reduce_to_index(tg_ctx* ctx, const tg_kv_desc* desc, const void* d_in, si
     const int p = ctx->nranks, me = ctx->rank;
     // the index range of this worker: Range(0, size).Partition(me, p) (common/math.hpp:85-94).  The limit is checked on the
     // largest range of any worker, so that every rank returns the same verdict.
-    auto range_begin = [&](u64 r) { return (u64)(((unsigned __int128)r * result_size + p - 1) / p); };
-    const u64 begin = range_begin(me), count = range_begin(me + 1) - begin;
+    const u64 begin = range_begin(me, result_size, p), count = range_begin(me + 1, result_size, p) - begin;
     u64 max_count = 0;
-    for (int r = 0; r < p; ++r) max_count = std::max(max_count, range_begin(r + 1) - range_begin(r));
+    for (int r = 0; r < p; ++r) max_count = std::max(max_count, range_begin(r + 1, result_size, p) - range_begin(r, result_size, p));
     if (max_count >= (1ull << 31)) return tg_set_error(ctx, TG_ERR_TOO_LARGE, "reduce_to_index: %llu indices per worker", (unsigned long long)max_count);
     // n_local >= 2^30: with several workers, the exchange reports it to every rank (a uniform TG_ERR_TOO_LARGE)
     const bool too_large = n_local >= (1u << 30);

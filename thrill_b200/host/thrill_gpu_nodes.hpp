@@ -7,6 +7,8 @@
  *     thrill_gpu::ReducePair(dia, std::plus<double> ...)          <->  DIA<T>::ReducePair(api/reduce_by_key.hpp:410)
  *     thrill_gpu::Merge(std::less<T>(), dia0, dia1, ...)          <->  api::Merge        (api/merge.hpp:673)
  *     thrill_gpu::InnerJoin(l, r, KeyFirst(), KeyFirst(), JoinValues()) <->  api::InnerJoin (api/inner_join.hpp:700)
+ *     thrill_gpu::GroupByKey<Out>(dia, KeyFirst(), fn)            <->  DIA<T>::GroupByKey (api/group_by_key.hpp:419)
+ *     thrill_gpu::GroupToIndex<Out>(dia, KeyFirst(), fn, size)    <->  DIA<T>::GroupToIndex (api/group_to_index.hpp:257)
  * Everything else of the pipeline (sources, LOps, other DOps, actions, the net/data layers) is the
  * UNMODIFIED reference library: this header only includes it.  The heavy lifting happens behind the C ABI
  * of include/thrill_gpu.h (libthrill_gpu.so): the nodes hand the Blocks of their input data::File to
@@ -717,6 +719,175 @@ private:
     bool have_host_file_ = false;
 };
 
+//! The iterator a GpuGroupNode hands to the group function: the public members of api::GroupByIterator
+//! (api/group_by_iterator.hpp:47-127), HasNext() and Next(), over the items of one group of the sorted host File.  The node
+//! drives it with the same two calls the stock nodes use (HasNextForReal, GetNextKey), so a function that stops before the end
+//! of its group is called again with the rest of it, as in the reference.
+template <typename ValueIn>
+class GroupIterator
+{
+public:
+    using Key = typename ValueIn::first_type;
+
+    explicit GroupIterator(thrill::data::File::Reader& reader)
+        : reader_(reader), elem_(reader_.template Next<ValueIn>()), key_(elem_.first) { }
+
+    GroupIterator(const GroupIterator&) = delete;
+    GroupIterator& operator = (const GroupIterator&) = delete;
+
+    bool HasNext() { return !is_reader_empty_ && equal_key_; }
+
+    ValueIn Next() {
+        assert(!is_reader_empty_);
+        ValueIn elem = elem_;
+        if (reader_.HasNext()) {
+            elem_ = reader_.template Next<ValueIn>();
+            if (elem_.first != key_) {
+                key_ = elem_.first;
+                equal_key_ = false;
+            }
+        }
+        else {
+            is_reader_empty_ = true;
+        }
+        return elem;
+    }
+
+    //! (the node's loop) items are left
+    bool HasNextForReal() const { return !is_reader_empty_; }
+    //! (the node's loop) the key of the next group; opens it for HasNext()
+    const Key& GetNextKey() {
+        equal_key_ = true;
+        return key_;
+    }
+
+private:
+    thrill::data::File::Reader& reader_;
+    bool is_reader_empty_ = false;
+    bool equal_key_ = true;
+    ValueIn elem_;
+    Key key_;
+};
+
+//! DIA::GroupByKey (api/group_by_key.hpp:46-428) and DIA::GroupToIndex (api/group_to_index.hpp:36-290) of a DIA of
+//! pair<uint64_t, 8-byte value> grouped by .first.  The exchange to the key's owner and the sort by the key run behind
+//! tg_group_by_key_file / tg_group_to_index_file (Execute, collective); PushData fetches the grouped items into a host File once
+//! and runs the stock nodes' RunUserFunc loop (group_by_key.hpp:314-331, group_to_index.hpp:186-215) over a GroupIterator.
+//! The group function and ValueOut are arbitrary, so the children get host items of ValueOut, never a device File.
+template <typename ValueOut, typename ValueIn, typename GroupFunction>
+class GpuGroupNode final : public thrill::api::DOpNode<ValueOut>, public GpuNodeBase
+{
+    using Super = thrill::api::DOpNode<ValueOut>;
+    using Super::context_;
+
+public:
+    //! to_index: GroupToIndex with result_size and neutral_element; otherwise GroupByKey
+    template <typename ParentDIA>
+    GpuGroupNode(const ParentDIA& parent, const GroupFunction& group_function, bool to_index, size_t result_size,
+                 const ValueOut& neutral_element)
+        : Super(parent.ctx(), to_index ? "GpuGroupToIndex" : "GpuGroupByKey", { parent.id() }, { parent.node() }),
+          group_function_(group_function), parent_stack_empty_(ParentDIA::stack_empty),
+          to_index_(to_index), result_size_(result_size), neutral_(neutral_element) {
+        auto pre_op_fn = [this](const ValueIn& input) { input_writer_.Put(input); };
+        auto lop_chain = parent.stack().push(pre_op_fn).fold();
+        parent.node()->AddChild(this, lop_chain);
+    }
+
+    DIAMemUse PreOpMemUse() final { return DIAMemUse::Max(); }
+
+    void StartPreOp(size_t /* parent_index */) final { input_writer_ = input_file_.GetWriter(); }
+
+    bool OnPreOpFile(const thrill::data::File& file, size_t /* parent_index */) final {
+        if (!parent_stack_empty_) return false;
+        input_file_ = file.Copy();
+        return true;
+    }
+
+    bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes, size_t /* parent_index */) final {
+        if (!parent_stack_empty_ || item_bytes != sizeof(ValueIn)) return false;
+        device_input_ = file;
+        return true;
+    }
+
+    void StopPreOp(size_t /* parent_index */) final { input_writer_.Close(); }
+
+    DIAMemUse ExecuteMemUse() final { return DIAMemUse::Max(); }
+
+    //! MainOp (group_by_key.hpp:348-376, group_to_index.hpp:234-254) behind tg_group_*_file.  Collective.  The grouped items
+    //! stay in HBM until PushData.
+    void Execute() final {
+        tg_ctx* c = WorkerCtx(context_);
+        std::unique_ptr<PinnedFileView> view;
+        tg_merge_input in;
+        if (device_input_) {
+            in = tg_merge_input { device_input_->get(), nullptr, 0 };
+        }
+        else {
+            view.reset(new PinnedFileView(input_file_, context_.local_worker_id()));
+            in = tg_merge_input { nullptr, view->data(), view->size() };
+        }
+        size_t out_items = 0;
+        if (to_index_)
+            Check(c, tg_group_to_index_file(c, &in, result_size_, &out_items, &range_begin_, &range_end_), "tg_group_to_index_file");
+        else
+            Check(c, tg_group_by_key_file(c, &in, &out_items), "tg_group_by_key_file");
+        view.reset();
+        input_file_.Clear();
+        device_input_.reset();
+        tg_dev_file f;
+        Check(c, tg_output_detach(c, &f), "tg_output_detach");
+        device_result_ = std::make_shared<DeviceFile>(c, f);
+        have_host_file_ = false;
+    }
+
+    DIAMemUse PushDataMemUse() final { return 0; }
+
+    //! RunUserFunc of the stock nodes over the grouped items.  They are fetched once and read without consuming them, so the
+    //! result can be pushed again until Dispose.  The key argument is the iterator's key, as in the stock nodes.
+    void PushData(bool /* consume */) final {
+        if (!have_host_file_) {
+            FetchDeviceFileIntoFile(WorkerCtx(context_), context_, *device_result_, sizeof(ValueIn), grouped_file_);
+            have_host_file_ = true;
+        }
+        auto r = grouped_file_.GetReader(/* consume */ false);
+        if (!to_index_) {
+            if (!r.HasNext()) return;
+            GroupIterator<ValueIn> it(r);
+            while (it.HasNextForReal())
+                this->PushItem(group_function_(it, it.GetNextKey()));
+            return;
+        }
+        size_t curr_index = range_begin_;
+        if (r.HasNext()) {
+            GroupIterator<ValueIn> it(r);
+            while (it.HasNextForReal()) {
+                if (it.GetNextKey() != curr_index) this->PushItem(neutral_);
+                else this->PushItem(group_function_(it, it.GetNextKey()));
+                ++curr_index;
+            }
+        }
+        while (curr_index < range_end_) {
+            this->PushItem(neutral_);
+            ++curr_index;
+        }
+    }
+
+    void Dispose() final { grouped_file_.Clear(); device_result_.reset(); have_host_file_ = false; }
+
+private:
+    GroupFunction group_function_;
+    const bool parent_stack_empty_;
+    const bool to_index_;
+    const size_t result_size_;
+    const ValueOut neutral_;
+    uint64_t range_begin_ = 0, range_end_ = 0;
+    thrill::data::File input_file_ { context_.GetFile(this) };
+    thrill::data::File::Writer input_writer_;
+    thrill::data::File grouped_file_ { context_.GetFile(this) };
+    DeviceFilePtr device_input_, device_result_;
+    bool have_host_file_ = false;
+};
+
 /******************************************************************************/
 // front doors (same argument meaning as DIA<T>::Sort / DIA<T>::ReducePair)
 
@@ -832,6 +1003,45 @@ auto InnerJoin(const LeftDIA& left, const RightDIA& right, const KeyFirst& /* ke
     auto node = tlx::make_counting<GpuJoinNode<ValueType, LeftType, RightType, JoinDesc<JoinFunction>::out_bytes> >(
         left, right, tg_join_desc { 16, JoinDesc<JoinFunction>::fn });
     return DIA<ValueType>(node);
+}
+
+//! the item types thrill_gpu::GroupByKey / GroupToIndex take: pair<uint64_t, 8-byte trivially copyable value>
+template <typename ValueIn>
+struct IsGroupPair : std::false_type { };
+template <typename V>
+struct IsGroupPair<std::pair<uint64_t, V> >
+    : std::integral_constant<bool, sizeof(V) == 8 && std::is_trivially_copyable<V>::value> { };
+
+//! DIA<T>::GroupByKey<ValueOut>(key_extractor, groupby_function) (api/group_by_key.hpp:419-428) for a DIA of pair<uint64_t,
+//! 8-byte value> grouped by .first (key_extractor KeyFirst).  group_function(iterator, key) is any function: it is called on the
+//! host once per group, with an iterator that has HasNext() and Next(), and returns a ValueOut.  Worker key % p holds a key's
+//! group (the stock placement with the default std::hash); groups come in ascending key order, the items of a group in global
+//! input order (one of the orders the stock operator allows).  Location detection and other hash functions are not offered.
+template <typename ValueOut, typename ValueIn, typename Stack, typename GroupFunction>
+auto GroupByKey(const DIA<ValueIn, Stack>& dia, const KeyFirst& /* key_extractor */, const GroupFunction& group_function) {
+    static_assert(IsGroupPair<ValueIn>::value,
+                  "thrill_gpu::GroupByKey: the DIA must hold pair<uint64_t, 8-byte value> grouped by KeyFirst; "
+                  "use the stock dia.GroupByKey<ValueOut>(key_extractor, group_function)");
+    assert(dia.IsValid());
+    auto node = tlx::make_counting<GpuGroupNode<ValueOut, ValueIn, GroupFunction> >(
+        dia, group_function, false, 0, ValueOut());
+    return DIA<ValueOut>(node);
+}
+
+//! DIA<T>::GroupToIndex<ValueOut>(key_extractor, groupby_function, size, neutral_element) (api/group_to_index.hpp:257-290) for a
+//! DIA of pair<uint64_t index, 8-byte value> grouped by .first: worker r pushes one ValueOut per index of
+//! Range(0, size).Partition(r, p), group_function(iterator, index) where the index has items and neutral_element where it has
+//! none.  An index >= size is an error (die) on every worker.
+template <typename ValueOut, typename ValueIn, typename Stack, typename GroupFunction>
+auto GroupToIndex(const DIA<ValueIn, Stack>& dia, const KeyFirst& /* key_extractor */, const GroupFunction& group_function,
+                  size_t size, const ValueOut& neutral_element = ValueOut()) {
+    static_assert(IsGroupPair<ValueIn>::value,
+                  "thrill_gpu::GroupToIndex: the DIA must hold pair<uint64_t, 8-byte value> grouped by KeyFirst; "
+                  "use the stock dia.GroupToIndex<ValueOut>(key_extractor, group_function, size)");
+    assert(dia.IsValid());
+    auto node = tlx::make_counting<GpuGroupNode<ValueOut, ValueIn, GroupFunction> >(
+        dia, group_function, true, size, neutral_element);
+    return DIA<ValueOut>(node);
 }
 
 } // namespace thrill_gpu
