@@ -24,7 +24,8 @@
  * and its _file form) takes at most 2^30 - 1 items per worker and side, before and after its exchange, and gives each worker at
  * most 2^30 - 1 items of the result.  GroupByKey and GroupToIndex (tg_group_by_key, tg_group_to_index and their _file forms)
  * take at most 2^30 - 1 items per worker, before and after their exchange, and tg_mod_partition at most 2^30 - 1 items per call.
- * The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
+ * PrefixSum, ExPrefixSum and ZipWithIndex (tg_prefix_sum, tg_zip_with_index, their _file and _select forms, tg_scan_local_total)
+ * take at most 2^30 - 1 items per worker and give each worker as many items as it holds.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
  ******************************************************************************/
 #ifndef THRILL_GPU_H
 #define THRILL_GPU_H
@@ -124,7 +125,8 @@ uint64_t tg_hot_records(const tg_ctx* ctx);
 enum { TG_K_RADIX_HIST = 0, TG_K_PARTITION = 1, TG_K_MERGE = 2, TG_K_PREAGG = 3, TG_K_AGGREGATE = 4,
        TG_K_COMPACT = 5, TG_K_OTHER = 6, TG_K_FIXUP = 7, TG_K_SEGCOUNT = 8,
        TG_K_EXCHANGE = 9 /* the NCCL Alltoallv (not a kernel of ours: timed like one) */,
-       TG_K_JOIN = 10 /* InnerJoin's co-rank count, offset scan and emit kernels */, TG_K_NUM = 11 };
+       TG_K_JOIN = 10 /* InnerJoin's co-rank count, offset scan and emit kernels */,
+       TG_K_SCAN = 11 /* PrefixSum's tile reduce, tile prefix and scan kernels; ZipWithIndex's kernel */, TG_K_NUM = 12 };
 int tg_profile_enable(tg_ctx* ctx, int on);
 int tg_profile_get(tg_ctx* ctx, int kernel_class, float* out_total_ms, uint64_t* out_launches);
 /* the individual launch durations of `kernel_class` in launch order (up to `capacity`); *out_n = how many there are */
@@ -396,6 +398,56 @@ int tg_group_to_index_file(tg_ctx* ctx, const tg_merge_input* in, uint64_t resul
 /* kernel level (tests of the placement on one GPU): GroupByKey's partition, destination of a 16-byte item = key % p.  Stable:
  * d_out receives the items grouped by destination in input order, out_counts[p] (host) the counts.  1 <= p <= 256. */
 int tg_mod_partition(tg_ctx* ctx, const void* d_in, size_t n, uint32_t p, void* d_out, uint64_t* out_counts);
+
+/* ---- PrefixSum / ExPrefixSum / ZipWithIndex: scans by global position (DIA::PrefixSum, DIA::ExPrefixSum, api/dia.hpp:1850,
+ * :1867, PrefixSumNode api/prefix_sum.hpp:28-128; DIA::ZipWithIndex, ZipWithIndexNode api/zip_with_index.hpp:40-110) -----------
+ * Every worker keeps its items, in order: one output per input item, no rebalancing (prefix_sum.hpp:92-110,
+ * zip_with_index.hpp:96-110).  The stock PrefixSumNode folds each worker's local total from the value-initialised item T(), not
+ * from the initial element: S_w = ((T() + x_0) + x_1) ... (prefix_sum.hpp:43, :56-59, :72-77), an empty worker contributes T().
+ * Worker r's carry is net.ExPrefixSum(S_r, +, initial) (:85-90), with thread workers on one host (net/flow_control_channel.hpp:
+ * 236-290) carry_0 = initial and carry_r = initial + (S_0 + ... + S_{r-1}), the inner fold left to right.  Then
+ *   inclusive  out_i = carry + x_0 + ... + x_i          exclusive  out_0 = carry, out_i = carry + x_0 + ... + x_{i-1}
+ * The descriptor set (the host shim recognises the sum function, thrill_b200/host/):
+ *   item_bytes 8   uint64_t with TG_OP_SUM_U64 (std::plus, wraps modulo 2^64), TG_OP_MIN_U64, TG_OP_MAX_U64 (thrill_gpu::MinU64 /
+ *                  MaxU64; with MinU64, T() = 0 absorbs everything, so every output of a worker r >= 1 is 0); double with
+ *                  TG_OP_SUM_F64 (std::plus<double>; local totals start from +0.0)
+ *   item_bytes 16  std::pair<uint64_t, V> (V any 8-byte value) with thrill_gpu::ScanSecond<F>: a + b = (b.first, F(a.second,
+ *                  b.second)), op = F's TG_OP_* as above.  So out_i.first is x_i.first (inclusive) or x_{i-1}.first (exclusive;
+ *                  carry.first for i = 0, which is the .first of worker r-1's last item, 0 if that worker is empty, and
+ *                  initial.first on worker 0)
+ * Anything else (TG_OP_MIN_F64, TG_OP_MAX_F64, TG_OP_FIRST, other item sizes) is TG_ERR_ARG.  Integer results are exact; double
+ * sums are bracketed by tiles (reduce-then-scan), the same way on every run, so a result is bitwise reproducible and differs from
+ * the stock left fold only by rounding.  The sign of a zero (-0.0 only where every summand is -0.0) is exact.
+ * ZipWithIndex takes 8-byte items (any value, copied as bits) and gives 16-byte pairs: index_first != 0 gives (index, item)
+ * (thrill_gpu::IndexFirst), index_first == 0 gives (item, index) (thrill_gpu::IndexSecond); index = the item's global position.
+ * Collective flow: p = 1 has no host round trip.  With p > 1 one ncclAllGather of a 32-byte record per worker (n_local and S_r)
+ * into device memory, then one host read of the gathered sizes: n_local >= 2^30 on any worker is TG_ERR_TOO_LARGE on every rank.
+ * The carry is folded on the device from the gathered totals; ZipWithIndex's base index is the sum of the lower ranks' sizes.
+ * Inputs are read, never modified.  Collective. */
+typedef struct {
+    uint32_t item_bytes;       /* 8 or 16 */
+    uint32_t op;               /* TG_OP_SUM_F64 (8-byte items only: double), TG_OP_SUM_U64, TG_OP_MIN_U64, TG_OP_MAX_U64 */
+} tg_scan_desc;
+/* on device buffers; initial_item: item_bytes bytes on the host (NULL: T(), all zero bytes); inclusive: PrefixSum (1) or
+ * ExPrefixSum (0).  *out_dptr holds n_local items, as for tg_sort (ctx-owned, valid until the next operator call). */
+int tg_prefix_sum(tg_ctx* ctx, const tg_scan_desc* desc, const void* d_in, size_t n_local, const void* initial_item,
+                  int inclusive, void** out_dptr, size_t* out_n);
+int tg_zip_with_index(tg_ctx* ctx, const void* d_in, size_t n_local, int index_first, void** out_dptr, size_t* out_n);
+/* the drop-in calls (GpuPrefixSumNode / GpuZipWithIndexNode::Execute): the input is a host File (Blocks) or a device File (read in
+ * place, left intact); the result is fetched with tg_fetch_output or taken with tg_output_detach */
+int tg_prefix_sum_file(tg_ctx* ctx, const tg_scan_desc* desc, const tg_merge_input* in, const void* initial_item, int inclusive,
+                       size_t* out_items);
+int tg_zip_with_index_file(tg_ctx* ctx, const tg_merge_input* in, int index_first, size_t* out_items);
+/* kernel level (p workers simulated on one GPU): the local total S of n items (what a worker contributes to the all-gather), as
+ * one item of desc->item_bytes bytes into host memory */
+int tg_scan_local_total(tg_ctx* ctx, const tg_scan_desc* desc, const void* d_in, size_t n, void* out_total_item);
+/* ... and worker `rank` of p (1 <= p <= 16): the operator's device path with totals (p items on the host, from
+ * tg_scan_local_total) in place of the all-gather, carry fold included; sizes[p] (host) are the workers' item counts, of which
+ * ZipWithIndex takes its base index.  Outputs as for tg_prefix_sum / tg_zip_with_index. */
+int tg_prefix_sum_select(tg_ctx* ctx, const tg_scan_desc* desc, const void* d_in, size_t n_local, uint32_t rank, uint32_t p,
+                         const void* totals, const void* initial_item, int inclusive, void** out_dptr, size_t* out_n);
+int tg_zip_with_index_select(tg_ctx* ctx, const void* d_in, size_t n_local, uint32_t rank, uint32_t p, const uint64_t* sizes,
+                             int index_first, void** out_dptr, size_t* out_n);
 
 /* ---- synthetic inputs of SURVEY.md §8(d), generated on the device (bench / tests support) ------------ */
 int tg_gen_sort_uniform(tg_ctx* ctx, void* d_out, uint64_t begin, uint64_t n, uint64_t seed);

@@ -8,6 +8,8 @@ Mirrors (same names, argument meaning and error behaviour) the slice of thrill/a
     DIA<T>::ReduceByKey(key_ex, reduce_fn) thrill/api/reduce_by_key.hpp:312-363
     DIA<T>::Merge(second, cmp) / api::Merge thrill/api/merge.hpp:674-721
     DIA<T>::GroupByKey / GroupToIndex      thrill/api/group_by_key.hpp:419-428, group_to_index.hpp:257-290
+    DIA<T>::PrefixSum / ExPrefixSum        thrill/api/dia.hpp:1850, :1867 (api/prefix_sum.hpp, ex_prefix_sum.hpp)
+    DIA<T>::ZipWithIndex(zip_function)     thrill/api/zip_with_index.hpp:140-152
     api::InnerJoin(l, r, key1, key2, fn)   thrill/api/inner_join.hpp:700-827
     DIA<T>::Size / AllGather / Gather      thrill/api/size.hpp, all_gather.hpp, gather.hpp
 A DIA here holds its local shard as a host numpy array — the stand-in for a data::File whose Blocks are
@@ -54,6 +56,21 @@ JoinKeyValues = _Functor("(l, r) -> tuple(l.first, l.second, r.second)", capi.JO
 JoinValues = _Functor("(l, r) -> pair(l.second, r.second)", capi.JOIN_VALUES)
 KEY_V1_V2 = np.dtype([("key", "<u8"), ("v1", "<u8"), ("v2", "<u8")])     # std::tuple<uint64_t, V1, V2>, member-wise
 V1_V2 = np.dtype([("v1", "<u8"), ("v2", "<u8")])                         # std::pair<V1, V2>
+
+
+def ScanSecond(value_function):
+    """thrill_gpu::ScanSecond<F>: the sum function of PrefixSum on pair<uint64_t, 8-byte value>, a + b = (b.first,
+    F(a.second, b.second)), with F one of PlusU64, MinU64, MaxU64, PlusDouble"""
+    if value_function not in (PlusU64, MinU64, MaxU64, PlusDouble):
+        raise capi.ThrillGpuError("ScanSecond: %r is not a sum function the GPU path recognises" % (value_function,))
+    f = _Functor("ScanSecond<%s>" % value_function.name, value_function.code)
+    f.on_second = True
+    return f
+
+
+# recognised zip functions of ZipWithIndex on 8-byte items: (index, item) or (item, index), as KV items
+IndexFirst = _Functor("(item, index) -> pair(index, item)")
+IndexSecond = _Functor("(item, index) -> pair(item, index)")
 
 
 def bind_to_gpu_numa_node(device):
@@ -374,6 +391,62 @@ class DIA(object):
         res = DIA(self.ctx, np.array(out, dtype=dtype))
         res.index_begin = begin
         return res
+
+    # ---- DIA<T>::PrefixSum / ExPrefixSum (api/prefix_sum.hpp:28-128) -------------------------------------------------------
+    def _scan_desc(self, what, sum_function):
+        it = self.items
+        if it.ndim == 1 and it.dtype == KV:
+            if sum_function is None or not getattr(sum_function, "on_second", False):
+                raise capi.ThrillGpuError("%s: pair items take ScanSecond(F) as the sum function" % what)
+            return capi.ScanDesc(16, sum_function.code)
+        if it.ndim == 1 and it.dtype == np.uint64:
+            fn = PlusU64 if sum_function is None else sum_function
+            if fn in (PlusU64, MinU64, MaxU64):
+                return capi.ScanDesc(8, fn.code)
+        if it.ndim == 1 and it.dtype == np.float64:
+            fn = PlusDouble if sum_function is None else sum_function
+            if fn is PlusDouble:
+                return capi.ScanDesc(8, fn.code)
+        raise capi.ThrillGpuError("%s: sum function %r on %r items is not one the GPU path recognises" % (what, sum_function, it.dtype))
+
+    def _prefix_sum(self, what, sum_function, initial_element, inclusive):
+        desc = self._scan_desc(what, sum_function)
+        if desc.item_bytes == 16:
+            ini = np.array(initial_element if initial_element is not None else (0, 0), np.uint64)
+        else:
+            ini = np.zeros(1, self.items.dtype)
+            if initial_element is not None:
+                ini[0] = initial_element
+        blocks, nb = self._blocks(self.items)
+        inp = capi.MergeInput(None, C.cast(blocks, C.POINTER(capi.Block)), nb)
+        n_out = C.c_size_t()
+        tg = self.ctx.tg
+        tg.ck(tg.L.tg_prefix_sum_file(tg.h, C.byref(desc), C.byref(inp), ini.ctypes.data, int(inclusive), C.byref(n_out)))
+        return DIA(self.ctx, self._fetch(n_out.value, self.items.dtype, desc.item_bytes))
+
+    def PrefixSum(self, sum_function=None, initial_element=None):
+        """out_i = carry + x_0 + ... + x_i on every worker, carry = initial_element + the local totals of the workers below
+        (each folded from T()).  uint64 items with PlusU64 (the default), MinU64 or MaxU64; float64 items with PlusDouble; KV
+        items with ScanSecond(F), initial_element a (first, second) tuple"""
+        return self._prefix_sum("PrefixSum", sum_function, initial_element, True)
+
+    def ExPrefixSum(self, sum_function=None, initial_element=None):
+        """out_0 = carry, out_i = carry + x_0 + ... + x_{i-1}; otherwise as PrefixSum"""
+        return self._prefix_sum("ExPrefixSum", sum_function, initial_element, False)
+
+    # ---- DIA<T>::ZipWithIndex (api/zip_with_index.hpp:40-152) -------------------------------------------------------------------
+    def ZipWithIndex(self, zip_function):
+        """8-byte items -> KV items: (global index, item bits) with IndexFirst, (item bits, global index) with IndexSecond"""
+        if zip_function not in (IndexFirst, IndexSecond):
+            raise capi.ThrillGpuError("ZipWithIndex: zip function %r is not one the GPU path recognises" % (zip_function,))
+        if not (self.items.ndim == 1 and self.items.dtype.itemsize == 8):
+            raise capi.ThrillGpuError("ZipWithIndex: items must be 8 bytes")
+        blocks, nb = self._blocks(self.items)
+        inp = capi.MergeInput(None, C.cast(blocks, C.POINTER(capi.Block)), nb)
+        n_out = C.c_size_t()
+        tg = self.ctx.tg
+        tg.ck(tg.L.tg_zip_with_index_file(tg.h, C.byref(inp), int(zip_function is IndexFirst), C.byref(n_out)))
+        return DIA(self.ctx, self._fetch(n_out.value, KV, 16))
 
     def ReduceByKey(self, key_extractor, reduce_function):
         if key_extractor is not KeyIsFirst:

@@ -12,7 +12,8 @@ LIB_PATH = os.environ.get("TG_LIB") or os.path.join(HERE, "csrc", "libthrill_gpu
 TG_OK = 0
 KEY_UINT_LE, KEY_BYTES_BE = 0, 1
 OP_SUM_F64, OP_SUM_U64, OP_MIN_U64, OP_MAX_U64, OP_MIN_F64, OP_MAX_F64, OP_FIRST = range(7)
-K_RADIX_HIST, K_PARTITION, K_MERGE, K_PREAGG, K_AGGREGATE, K_COMPACT, K_OTHER, K_FIXUP, K_SEGCOUNT, K_EXCHANGE, K_JOIN = range(11)
+K_RADIX_HIST, K_PARTITION, K_MERGE, K_PREAGG, K_AGGREGATE, K_COMPACT, K_OTHER, K_FIXUP, K_SEGCOUNT, K_EXCHANGE, K_JOIN, K_SCAN = \
+    range(12)
 JOIN_KEY_VALUES, JOIN_VALUES = 0, 1
 
 
@@ -40,6 +41,10 @@ class MergeInput(C.Structure):
 
 class JoinDesc(C.Structure):
     _fields_ = [("item_bytes", C.c_uint32), ("join_fn", C.c_uint32)]
+
+
+class ScanDesc(C.Structure):
+    _fields_ = [("item_bytes", C.c_uint32), ("op", C.c_uint32)]
 
 
 class BlockGeom(C.Structure):
@@ -126,6 +131,13 @@ SYMBOLS = [
     ("tg_group_by_key_file", _i, [_vp, _P(MergeInput), _P(_sz)]),
     ("tg_group_to_index_file", _i, [_vp, _P(MergeInput), _u64, _P(_sz), _P(_u64), _P(_u64)]),
     ("tg_mod_partition", _i, [_vp, _vp, _sz, _u32, _vp, _P(_u64)]),
+    ("tg_prefix_sum", _i, [_vp, _P(ScanDesc), _vp, _sz, _vp, _i, _P(_vp), _P(_sz)]),
+    ("tg_zip_with_index", _i, [_vp, _vp, _sz, _i, _P(_vp), _P(_sz)]),
+    ("tg_prefix_sum_file", _i, [_vp, _P(ScanDesc), _P(MergeInput), _vp, _i, _P(_sz)]),
+    ("tg_zip_with_index_file", _i, [_vp, _P(MergeInput), _i, _P(_sz)]),
+    ("tg_scan_local_total", _i, [_vp, _P(ScanDesc), _vp, _sz, _vp]),
+    ("tg_prefix_sum_select", _i, [_vp, _P(ScanDesc), _vp, _sz, _u32, _u32, _vp, _vp, _i, _P(_vp), _P(_sz)]),
+    ("tg_zip_with_index_select", _i, [_vp, _vp, _sz, _u32, _u32, _P(_u64), _i, _P(_vp), _P(_sz)]),
     ("tg_transfer_bytes", _i, [_vp, _P(_u64), _P(_u64)]),
     ("tg_gen_sort_uniform", _i, [_vp, _vp, _u64, _u64, _u64]),
     ("tg_gen_reduce_uniform", _i, [_vp, _vp, _u64, _u64, _u64, _u64, _i]),

@@ -15,7 +15,7 @@
 typedef unsigned long long u64;
 typedef unsigned int u32;
 
-#define TG_NUM_WS 25
+#define TG_NUM_WS 27
 #define TG_MAX_RANKS 16
 
 struct tg_ctx {
@@ -72,7 +72,9 @@ enum { WS_SORT_TMP = 0, WS_SORT_STATUS = 1, WS_SORT_HIST = 2, WS_XCHG_SEND = 3, 
        WS_SORT_HIST2 = 15, WS_SEG_TILES2 = 16, WS_DENSE = 17, WS_XCTL = 18, WS_REC = 19, WS_HOT = 20,
        // InnerJoin (tg_join.cu): the sorted sides (items + sort scratch each), counts / offsets / splits, the output.
        // GroupByKey / GroupToIndex (tg_group.cu) sort into WS_JOIN_L: their result is the sorted items
-       WS_JOIN_L = 21, WS_JOIN_R = 22, WS_JOIN_AUX = 23, WS_JOIN_OUT = 24 };
+       WS_JOIN_L = 21, WS_JOIN_R = 22, WS_JOIN_AUX = 23, WS_JOIN_OUT = 24,
+       // PrefixSum / ExPrefixSum / ZipWithIndex (tg_scan.cu): tile aggregates, prefixes and the gathered records; the output
+       WS_SCAN_AUX = 25, WS_SCAN_OUT = 26 };
 
 int tg_set_error(tg_ctx* ctx, int status, const char* fmt, ...);
 int tg_ws_get(tg_ctx* ctx, int slot, size_t bytes, void** out);

@@ -9,6 +9,8 @@
  *     thrill_gpu::InnerJoin(l, r, KeyFirst(), KeyFirst(), JoinValues()) <->  api::InnerJoin (api/inner_join.hpp:700)
  *     thrill_gpu::GroupByKey<Out>(dia, KeyFirst(), fn)            <->  DIA<T>::GroupByKey (api/group_by_key.hpp:419)
  *     thrill_gpu::GroupToIndex<Out>(dia, KeyFirst(), fn, size)    <->  DIA<T>::GroupToIndex (api/group_to_index.hpp:257)
+ *     thrill_gpu::PrefixSum(dia, fn [, initial]) / ExPrefixSum    <->  DIA<T>::PrefixSum / ExPrefixSum (api/dia.hpp:1850, :1867)
+ *     thrill_gpu::ZipWithIndex(dia, IndexFirst() | IndexSecond()) <->  DIA<T>::ZipWithIndex (api/zip_with_index.hpp:140)
  * Everything else of the pipeline (sources, LOps, other DOps, actions, the net/data layers) is the
  * UNMODIFIED reference library: this header only includes it.  The heavy lifting happens behind the C ABI
  * of include/thrill_gpu.h (libthrill_gpu.so): the nodes hand the Blocks of their input data::File to
@@ -222,6 +224,45 @@ template <>
 struct JoinDesc<JoinValues>{
     static constexpr bool supported = true;
     static constexpr uint32_t fn = TG_JOIN_VALUES, out_bytes = 16;
+};
+
+//! The sum function thrill_gpu::PrefixSum / ExPrefixSum recognise on pair<uint64_t, V>: F (one of the ReducePair functions,
+//! std::plus<double>, std::plus<uint64_t>, MinU64, MaxU64) on .second, .first taken from the right-hand operand.  Prefix doubling
+//! names its suffixes with ScanSecond<MaxU64> (examples/suffix_sorting/prefix_doubling.cpp:348).  A plain functor with one
+//! operator() (the stock nodes read its argument type), so the stock DIA::PrefixSum takes it too.
+template <typename MemberFn> struct MemberResult;
+template <typename R, typename C, typename... A>
+struct MemberResult<R (C::*)(A...) const> { using type = R; };
+template <typename ValueFunction>
+struct ScanSecond {
+    using Pair = std::pair<uint64_t, typename MemberResult<decltype(&ValueFunction::operator ())>::type>;
+    ValueFunction fn;
+    Pair operator () (const Pair& a, const Pair& b) const { return Pair(b.first, fn(a.second, b.second)); }
+};
+//! the (item type, sum function) pairs of PrefixSum / ExPrefixSum: uint64_t and double with their ReduceDesc functions, and
+//! pair<uint64_t, V> with ScanSecond<F>
+template <typename Value, typename SumFunction, bool = ReduceDesc<Value, SumFunction>::supported>
+struct ScanOp { static constexpr bool supported = false; static constexpr uint32_t op = 0; };
+template <typename Value, typename SumFunction>
+struct ScanOp<Value, SumFunction, true>{
+    static constexpr bool supported = true;
+    static constexpr uint32_t op = ReduceDesc<Value, SumFunction>::op;
+};
+template <typename ValueType, typename SumFunction>
+struct ScanDesc : ScanOp<ValueType, SumFunction> { static constexpr uint32_t item_bytes = 8; };
+template <typename V, typename F>
+struct ScanDesc<std::pair<uint64_t, V>, ScanSecond<F> >
+    : ScanOp<typename std::conditional<std::is_same<V, typename ScanSecond<F>::Pair::second_type>::value, V, void>::type, F>{
+    static constexpr uint32_t item_bytes = 16;
+};
+//! The zip functions thrill_gpu::ZipWithIndex recognises on 8-byte items: (item, index) -> pair(index, item) or pair(item, index)
+struct IndexFirst {
+    template <typename T>
+    std::pair<uint64_t, T> operator () (const T& item, const size_t& index) const { return std::pair<uint64_t, T>(index, item); }
+};
+struct IndexSecond {
+    template <typename T>
+    std::pair<T, uint64_t> operator () (const T& item, const size_t& index) const { return std::pair<T, uint64_t>(item, index); }
 };
 
 /******************************************************************************/
@@ -888,6 +929,109 @@ private:
     bool have_host_file_ = false;
 };
 
+//! DIA::PrefixSum / DIA::ExPrefixSum (PrefixSumNode, api/prefix_sum.hpp:28-128) and DIA::ZipWithIndex (ZipWithIndexNode,
+//! api/zip_with_index.hpp:40-128): the stock node protocol (a File of the parent's items, or the parent's File whole through
+//! OnPreOpFile) with the collective call in Execute: tg_prefix_sum_file (the all-gather of the local totals, the carry and the
+//! scan) or tg_zip_with_index_file.  The input may arrive as a device File from a parent GPU node, and the result, one item per
+//! input item on the same worker, is handed to GPU children in HBM.  zip: ZipWithIndex with index_first; otherwise PrefixSum
+//! with desc, initial and inclusive.
+template <typename ValueOut, typename ValueIn>
+class GpuScanNode final : public thrill::api::DOpNode<ValueOut>, public GpuNodeBase
+{
+    using Super = thrill::api::DOpNode<ValueOut>;
+    using Super::context_;
+
+public:
+    template <typename ParentDIA>
+    GpuScanNode(const ParentDIA& parent, const char* label, bool zip, const tg_scan_desc& desc, const ValueIn& initial,
+                bool inclusive, bool index_first)
+        : Super(parent.ctx(), label, { parent.id() }, { parent.node() }),
+          zip_(zip), desc_(desc), initial_(initial), inclusive_(inclusive), index_first_(index_first),
+          parent_stack_empty_(ParentDIA::stack_empty) {
+        auto pre_op_fn = [this](const ValueIn& input) { input_writer_.Put(input); };
+        auto lop_chain = parent.stack().push(pre_op_fn).fold();
+        parent.node()->AddChild(this, lop_chain);
+    }
+
+    void StartPreOp(size_t /* parent_index */) final { input_writer_ = input_file_.GetWriter(); }
+
+    bool OnPreOpFile(const thrill::data::File& file, size_t /* parent_index */) final {
+        if (!parent_stack_empty_) return false;
+        input_file_ = file.Copy();
+        return true;
+    }
+
+    bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes, size_t /* parent_index */) final {
+        if (!parent_stack_empty_ || item_bytes != sizeof(ValueIn)) return false;
+        device_input_ = file;
+        return true;
+    }
+
+    void StopPreOp(size_t /* parent_index */) final { input_writer_.Close(); }
+
+    DIAMemUse ExecuteMemUse() final { return DIAMemUse::Max(); }
+
+    //! Execute (prefix_sum.hpp:84-90, zip_with_index.hpp:86-94) and the outputs of PushData behind one call.  Collective.
+    void Execute() final {
+        tg_ctx* c = WorkerCtx(context_);
+        std::unique_ptr<PinnedFileView> view;
+        tg_merge_input in;
+        if (device_input_) {
+            in = tg_merge_input { device_input_->get(), nullptr, 0 };
+        }
+        else {
+            view.reset(new PinnedFileView(input_file_, context_.local_worker_id()));
+            in = tg_merge_input { nullptr, view->data(), view->size() };
+        }
+        size_t out_items = 0;
+        if (zip_)
+            Check(c, tg_zip_with_index_file(c, &in, index_first_ ? 1 : 0, &out_items), "tg_zip_with_index_file");
+        else
+            Check(c, tg_prefix_sum_file(c, &desc_, &in, &initial_, inclusive_ ? 1 : 0, &out_items), "tg_prefix_sum_file");
+        view.reset();
+        input_file_.Clear();
+        device_input_.reset();
+        tg_dev_file f;
+        Check(c, tg_output_detach(c, &f), "tg_output_detach");
+        device_result_ = std::make_shared<DeviceFile>(c, f);
+        have_host_file_ = false;
+    }
+
+    DIAMemUse PushDataMemUse() final { return 0; }
+
+    void PushData(bool consume) final {
+        if (device_result_ && AllChildrenAreGpuNodes(*this)) {
+            bool all = true;
+            for (const auto& ch : this->children_)
+                all = dynamic_cast<GpuNodeBase*>(ch.node)->OnPreOpDeviceFile(device_result_, sizeof(ValueOut), ch.parent_index) && all;
+            if (all) return;
+        }
+        if (!have_host_file_) {
+            FetchDeviceFileIntoFile(WorkerCtx(context_), context_, *device_result_, sizeof(ValueOut), result_file_);
+            have_host_file_ = true;
+        }
+        this->PushFile(result_file_, consume);
+    }
+
+    void Dispose() final { result_file_.Clear(); device_result_.reset(); have_host_file_ = false; }
+
+private:
+    const bool zip_;
+    const tg_scan_desc desc_;
+    const ValueIn initial_;
+    const bool inclusive_, index_first_;
+    const bool parent_stack_empty_;
+    thrill::data::File input_file_ { context_.GetFile(this) };
+    thrill::data::File::Writer input_writer_;
+    thrill::data::File result_file_ { context_.GetFile(this) };
+    DeviceFilePtr device_input_, device_result_;
+    bool have_host_file_ = false;
+};
+template <typename ValueType>
+using GpuPrefixSumNode = GpuScanNode<ValueType, ValueType>;
+template <typename ValueOut, typename ValueIn>
+using GpuZipWithIndexNode = GpuScanNode<ValueOut, ValueIn>;
+
 /******************************************************************************/
 // front doors (same argument meaning as DIA<T>::Sort / DIA<T>::ReducePair)
 
@@ -1041,6 +1185,58 @@ auto GroupToIndex(const DIA<ValueIn, Stack>& dia, const KeyFirst& /* key_extract
     assert(dia.IsValid());
     auto node = tlx::make_counting<GpuGroupNode<ValueOut, ValueIn, GroupFunction> >(
         dia, group_function, true, size, neutral_element);
+    return DIA<ValueOut>(node);
+}
+
+//! DIA<T>::PrefixSum(sum_function, initial_element) (api/dia.hpp:1850, api/prefix_sum.hpp:132-160) for the recognised pairs:
+//! uint64_t with std::plus<uint64_t>, MinU64 or MaxU64; double with std::plus<double>; pair<uint64_t, V> with ScanSecond<F>.
+//! out_i = carry + x_0 + ... + x_i, carry = initial_element + the local totals of the workers below (each folded from T()),
+//! as in the stock node.  Items stay on their worker.  Double sums are bracketed by tiles: reproducible, equal to the stock
+//! left fold up to rounding.
+template <typename ValueType, typename Stack, typename SumFunction>
+auto PrefixSum(const DIA<ValueType, Stack>& dia, const SumFunction& /* sum_function */,
+               const typename DIA<ValueType, Stack>::ValueType& initial_element = ValueType()) {
+    static_assert(ScanDesc<ValueType, SumFunction>::supported,
+                  "thrill_gpu::PrefixSum: this (ValueType, SumFunction) pair has no GPU descriptor; "
+                  "use the stock dia.PrefixSum(sum_function, initial_element)");
+    assert(dia.IsValid());
+    auto node = tlx::make_counting<GpuPrefixSumNode<ValueType> >(
+        dia, "GpuPrefixSum", false,
+        tg_scan_desc { ScanDesc<ValueType, SumFunction>::item_bytes, ScanDesc<ValueType, SumFunction>::op },
+        initial_element, true, false);
+    return DIA<ValueType>(node);
+}
+
+//! DIA<T>::ExPrefixSum(sum_function, initial_element) (api/dia.hpp:1867, api/ex_prefix_sum.hpp): out_0 = carry,
+//! out_i = carry + x_0 + ... + x_{i-1}; otherwise as PrefixSum
+template <typename ValueType, typename Stack, typename SumFunction>
+auto ExPrefixSum(const DIA<ValueType, Stack>& dia, const SumFunction& /* sum_function */,
+                 const typename DIA<ValueType, Stack>::ValueType& initial_element = ValueType()) {
+    static_assert(ScanDesc<ValueType, SumFunction>::supported,
+                  "thrill_gpu::ExPrefixSum: this (ValueType, SumFunction) pair has no GPU descriptor; "
+                  "use the stock dia.ExPrefixSum(sum_function, initial_element)");
+    assert(dia.IsValid());
+    auto node = tlx::make_counting<GpuPrefixSumNode<ValueType> >(
+        dia, "GpuExPrefixSum", false,
+        tg_scan_desc { ScanDesc<ValueType, SumFunction>::item_bytes, ScanDesc<ValueType, SumFunction>::op },
+        initial_element, false, false);
+    return DIA<ValueType>(node);
+}
+
+//! DIA<T>::ZipWithIndex(zip_function) (api/zip_with_index.hpp:140-152) of 8-byte trivially copyable items with
+//! zip_function IndexFirst (-> pair<uint64_t, T>(index, item), the input of ReduceToIndex / GroupToIndex) or IndexSecond
+//! (-> pair<T, uint64_t>(item, index), the (char, index) tuples of the suffix sorters).  Items stay on their worker.
+template <typename ValueType, typename Stack, typename ZipFunction>
+auto ZipWithIndex(const DIA<ValueType, Stack>& dia, const ZipFunction& zip_function) {
+    static_assert((std::is_same<ZipFunction, IndexFirst>::value || std::is_same<ZipFunction, IndexSecond>::value) &&
+                  sizeof(ValueType) == 8 && std::is_trivially_copyable<ValueType>::value,
+                  "thrill_gpu::ZipWithIndex: 8-byte items with IndexFirst or IndexSecond only; "
+                  "use the stock dia.ZipWithIndex(zip_function)");
+    assert(dia.IsValid());
+    using ValueOut = decltype(zip_function(std::declval<ValueType>(), size_t(0)));
+    auto node = tlx::make_counting<GpuZipWithIndexNode<ValueOut, ValueType> >(
+        dia, "GpuZipWithIndex", true, tg_scan_desc { 8, 0 }, ValueType(), true,
+        std::is_same<ZipFunction, IndexFirst>::value);
     return DIA<ValueOut>(node);
 }
 
