@@ -1,8 +1,8 @@
 """Worker of test_gpu_scan.py::test_scan_on_n_gpus: one process per GPU (torchrun), runs tg_prefix_sum / tg_zip_with_index on
 shards placed as the reference's workers held them and checks this worker's rows against the reference's worker `rank` at
-p = world in tests/golden/reference_outputs_scan.npz (uneven and empty shards included; double sums within the tolerance of
-test_gpu_scan.py), then a shard of a real 2^30-item buffer on rank 0: TG_ERR_TOO_LARGE on every rank.  Exit code 0 and
-MULTI_GPU_SCAN_OK = parity."""
+p = world in tests/golden/reference_outputs_scan.npz (uneven and empty shards included; double sums against the exact
+prefix sums within the rounding bound of scan_exact.py), then a shard of a real 2^30-item buffer on rank 0:
+TG_ERR_TOO_LARGE on every rank.  Exit code 0 and MULTI_GPU_SCAN_OK = parity."""
 import ctypes as C
 import os
 import sys
@@ -16,8 +16,8 @@ sys.path.insert(0, HERE)
 import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
 
+import scan_exact as X  # noqa: E402
 import scan_ref as S  # noqa: E402
-from test_gpu_scan import assert_f64_close  # noqa: E402
 from thrill_b200 import api, capi  # noqa: E402
 
 GOLDEN = os.path.join(HERE, "golden", "reference_outputs_scan.npz")
@@ -61,9 +61,8 @@ def main():
         rows[:, 0] = rank
         if case.op == S.OP_SUM_F64:
             assert np.array_equal(rows[:, :2], ref[:, :2]), name
-            init = float(np.array([case.initial[1]], np.uint64).view(np.float64)[0])
-            scale = S.f64_abs_prefix(case.shards(world), case.pair, init)[rank]
-            assert_f64_close(rows[:, 2], ref[:, 2], scale)
+            X.check(rows[:, 2], case.shards(world), case.pair, case.initial, case.inclusive, stock=ref[:, 2],
+                    select=np.arange(lo, lo + counts[rank]))
         else:
             assert S.rows_equal(rows, ref), (name, rank)
         checked += 1

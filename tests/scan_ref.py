@@ -156,18 +156,6 @@ def pairs(first, second):
     return out
 
 
-def f64_abs_prefix(shards, pair=False, initial=0.0):
-    """the same inclusive prefix over |x| (and |initial|), the scale of the rounding error of a double sum"""
-    a = [np.abs(split_values(s, pair)[1].view(np.float64)) for s in shards]
-    allv = np.concatenate([[abs(initial)]] + a)
-    acc = np.add.accumulate(allv)
-    outs, pos = [], 1
-    for x in a:
-        outs.append(acc[pos:pos + len(x)])
-        pos += len(x)
-    return outs
-
-
 # ---- the fixtures of tests/golden/make_golden_scan.py ------------------------------------------------------------------------
 MODES = ["sum_u64", "min_u64", "max_u64", "sum_f64", "pair_max", "pair_sum_f64", "zip_first", "zip_second"]
 MODE_OP = {"sum_u64": OP_SUM_U64, "min_u64": OP_MIN_U64, "max_u64": OP_MAX_U64, "sum_f64": OP_SUM_F64,

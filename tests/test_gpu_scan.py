@@ -1,9 +1,10 @@
 """PrefixSum / ExPrefixSum / ZipWithIndex on one H100: tg_prefix_sum, tg_zip_with_index, their _file and _select forms,
 tg_scan_local_total and the Python mirror against the numpy restatement in scan_ref.py and against the reference's outputs in
 tests/golden/reference_outputs_scan.npz, including p = 2, 3, 4, 8 and 16 workers simulated on one GPU through the kernel-level
-entries.  Integer results are compared bit for bit; double sums (bracketed by tiles, not left to right) within
-1e-9 * max(1, the prefix over |x|), with NaN, inf and the sign of zero exact.  Tile edges, device Files, argument errors, the size
-limit, full-size cases, the multi-GPU worker and the in-Thrill test binary where the machine has what they need.  pytest -m gpu."""
+entries.  Integer results are compared bit for bit; double sums (bracketed by tiles, not left to right) against the exact
+prefix sums within the rounding bound of the bracketing (scan_exact.py), with NaN, inf and the sign of zero exact.  Tile
+edges, device Files, argument errors, the size limit, full-size cases, the multi-GPU worker and the in-Thrill test binary
+where the machine has what they need.  pytest -m gpu."""
 import ctypes as C
 import os
 import subprocess
@@ -12,6 +13,7 @@ import sys
 import numpy as np
 import pytest
 
+import scan_exact as X
 import scan_ref as S
 from gpu_util import make_blocks
 
@@ -78,23 +80,6 @@ def words(a):
     return np.ascontiguousarray(a).view(np.uint64).reshape(-1)
 
 
-def values(a, pair):
-    return words(a).reshape(-1, 2)[:, 1] if pair else words(a)
-
-
-def assert_f64_close(got, ref, scale):
-    """got, ref: double bits; NaN, inf and the sign of a zero exact, the rest within 1e-9 * max(1, scale)"""
-    g, r = np.asarray(got, np.uint64).view(np.float64), np.asarray(ref, np.uint64).view(np.float64)
-    assert np.array_equal(np.isnan(g), np.isnan(r))
-    inf = np.isinf(r)
-    assert np.array_equal(g[inf], r[inf]) and not np.isinf(g[~inf]).any()
-    both0 = (g == 0) & (r == 0)
-    assert np.array_equal(np.signbit(g[both0]), np.signbit(r[both0]))
-    fin = np.isfinite(r)
-    tol = 1e-9 * np.maximum(1.0, np.asarray(scale, np.float64)[fin])
-    assert (np.abs(g[fin] - r[fin]) <= tol).all(), float(np.max(np.abs(g[fin] - r[fin]) - tol))
-
-
 def check(ctx, items, op, pair=False, initial=(0, 0), inclusive=True):
     st, res = scan_dev(ctx, items, op, pair, initial, inclusive)
     assert st == 0, ctx.L.tg_last_error(ctx.h)
@@ -102,8 +87,7 @@ def check(ctx, items, op, pair=False, initial=(0, 0), inclusive=True):
     if pair:
         assert np.array_equal(res["key"], ref["key"])
     if op == S.OP_SUM_F64:
-        scale = S.f64_abs_prefix([items], pair, float(np.array([initial[1]], np.uint64).view(np.float64)[0]))[0]
-        assert_f64_close(values(res, pair), values(ref, pair), scale)
+        X.check([res], [items], pair, initial, inclusive)
     else:
         assert np.array_equal(words(res), words(ref))
     return res
@@ -200,8 +184,11 @@ def test_local_total(ctx):
                 ctx.free(d)
                 ref = S.totals_of([items], op, pair)[0]
                 if op == S.OP_SUM_F64:
-                    scale = S.f64_abs_prefix([items], pair)[0]
-                    assert_f64_close(tot[-1:], [ref[1] if pair else ref], scale[-1:] if n else [0.0])
+                    # S = T() + x_0 + ... : the inclusive prefix at the last item (+0.0, T(), when there is none)
+                    if n:
+                        X.check(tot[-1:], [items], pair, (0, 0), True, select=[n - 1])
+                    else:
+                        assert int(tot[-1]) == 0
                     if pair:
                         assert int(tot[0]) == ref[0]
                 else:
@@ -253,9 +240,8 @@ def check_rows(case, p, outs, ref_rows):
         assert S.rows_equal(rows, ref_rows), (case.name, p)
         return
     assert np.array_equal(rows[:, :2], ref_rows[:, :2]), (case.name, p)
-    init = float(np.array([case.initial[1]], np.uint64).view(np.float64)[0])
-    scale = np.concatenate(S.f64_abs_prefix(case.shards(p), case.pair, init))
-    assert_f64_close(rows[:, 2], ref_rows[:, 2], scale)
+    # the stock's stored outputs give NaN, inf and the signs of zeros; the finite values are checked against the exact sums
+    X.check(rows[:, 2], case.shards(p), case.pair, case.initial, case.inclusive, stock=ref_rows[:, 2])
 
 
 @pytest.mark.parametrize("p", [1, 2, 3, 4, 8])
@@ -296,9 +282,7 @@ def test_sixteen_simulated_workers(ctx, op):
                 if op != S.OP_SUM_F64:
                     assert np.array_equal(words(o), words(r))
             if op == S.OP_SUM_F64:
-                scale = np.concatenate(S.f64_abs_prefix(shards, pair, float(np.array([9], np.uint64).view(np.float64)[0])))
-                assert_f64_close(np.concatenate([values(o, pair) for o in outs]),
-                                 np.concatenate([values(r, pair) for r in ref]), scale)
+                X.check(outs, shards, pair, (42, 9), inclusive)
     x = gen_u64(50000, 3)
     shards = S.shards_of(x, [3000 * (r % 3) for r in range(15)] + [50000 - sum(3000 * (r % 3) for r in range(15))])
     for first in (True, False):

@@ -1191,8 +1191,8 @@ auto GroupToIndex(const DIA<ValueIn, Stack>& dia, const KeyFirst& /* key_extract
 //! DIA<T>::PrefixSum(sum_function, initial_element) (api/dia.hpp:1850, api/prefix_sum.hpp:132-160) for the recognised pairs:
 //! uint64_t with std::plus<uint64_t>, MinU64 or MaxU64; double with std::plus<double>; pair<uint64_t, V> with ScanSecond<F>.
 //! out_i = carry + x_0 + ... + x_i, carry = initial_element + the local totals of the workers below (each folded from T()),
-//! as in the stock node.  Items stay on their worker.  Double sums are bracketed by tiles: reproducible, equal to the stock
-//! left fold up to rounding.
+//! as in the stock node.  Items stay on their worker.  Double sums are bracketed by tiles: bitwise reproducible, and within
+//! the rounding bound of tg_prefix_sum (include/thrill_gpu.h) of the exact sums while no partial sum can overflow.
 template <typename ValueType, typename Stack, typename SumFunction>
 auto PrefixSum(const DIA<ValueType, Stack>& dia, const SumFunction& /* sum_function */,
                const typename DIA<ValueType, Stack>::ValueType& initial_element = ValueType()) {
