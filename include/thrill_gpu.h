@@ -25,7 +25,8 @@
  * most 2^30 - 1 items of the result.  GroupByKey and GroupToIndex (tg_group_by_key, tg_group_to_index and their _file forms)
  * take at most 2^30 - 1 items per worker, before and after their exchange, and tg_mod_partition at most 2^30 - 1 items per call.
  * PrefixSum, ExPrefixSum and ZipWithIndex (tg_prefix_sum, tg_zip_with_index, their _file and _select forms, tg_scan_local_total)
- * take at most 2^30 - 1 items per worker and give each worker as many items as it holds.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
+ * take at most 2^30 - 1 items per worker and give each worker as many items as it holds.  Sum, Min, Max and AllReduce (tg_all_reduce
+ * and its _file and _select forms) take at most 2^30 - 1 items per worker.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
  ******************************************************************************/
 #ifndef THRILL_GPU_H
 #define THRILL_GPU_H
@@ -126,7 +127,8 @@ enum { TG_K_RADIX_HIST = 0, TG_K_PARTITION = 1, TG_K_MERGE = 2, TG_K_PREAGG = 3,
        TG_K_COMPACT = 5, TG_K_OTHER = 6, TG_K_FIXUP = 7, TG_K_SEGCOUNT = 8,
        TG_K_EXCHANGE = 9 /* the NCCL Alltoallv (not a kernel of ours: timed like one) */,
        TG_K_JOIN = 10 /* InnerJoin's co-rank count, offset scan and emit kernels */,
-       TG_K_SCAN = 11 /* PrefixSum's tile reduce, tile prefix and scan kernels; ZipWithIndex's kernel */, TG_K_NUM = 12 };
+       TG_K_SCAN = 11 /* PrefixSum's tile reduce, tile prefix and scan kernels; ZipWithIndex's kernel; the actions' tile reduce
+                         and fold */, TG_K_NUM = 12 };
 int tg_profile_enable(tg_ctx* ctx, int on);
 int tg_profile_get(tg_ctx* ctx, int kernel_class, float* out_total_ms, uint64_t* out_launches);
 /* the individual launch durations of `kernel_class` in launch order (up to `capacity`); *out_n = how many there are */
@@ -455,6 +457,54 @@ int tg_prefix_sum_select(tg_ctx* ctx, const tg_scan_desc* desc, const void* d_in
                          const void* totals, const void* initial_item, int inclusive, void** out_dptr, size_t* out_n);
 int tg_zip_with_index_select(tg_ctx* ctx, const void* d_in, size_t n_local, uint32_t rank, uint32_t p, const uint64_t* sizes,
                              int index_first, void** out_dptr, size_t* out_n);
+
+/* ---- Sum / Min / Max / AllReduce: a DIA reduced to one value on every worker (DIA::Sum, Min, Max, AllReduce: api/sum.hpp,
+ * min.hpp, max.hpp, AllReduceNode api/all_reduce.hpp:27-85) ---------------------------------------------------------------------
+ * Worker value S_r: the worker folds its items left to right starting from its FIRST item, not from an identity
+ * (all_reduce.hpp:56-63): S_r = ((x_0 + x_1) + x_2) ...  With an initial value (Sum(fn, initial), Min(initial), Max(initial),
+ * AllReduce(fn, initial)) worker 0 starts from it instead and folds every item into it.  A worker with no items contributes T(),
+ * the value-initialised item (0, +0.0, (0, 0)), or, when there is an initial value, the initial value: the stock node's value
+ * starts as the initial value on every worker, and a worker other than 0 replaces it with its first item (:39-46).  So with an
+ * empty worker the Min() of positive uint64_t values is 0, the Min() of doubles is at most +0.0, and Sum(fn, initial) counts the
+ * initial value once more for every empty worker other than worker 0, exactly as in the stock node.
+ * Result: the left fold of the worker values in rank order, v = S_0, v = v + S_r for r = 1..p-1 (FlowControlChannel::AllReduce
+ * with the thread workers of one host, net/flow_control_channel.hpp:599-638); every rank gets the same value.
+ * The descriptor set (tg_scan_desc; the host shim recognises the function, thrill_b200/host/):
+ *   item_bytes 8   uint64_t with TG_OP_SUM_U64 (std::plus, wraps modulo 2^64), TG_OP_MIN_U64 (thrill_gpu::MinU64,
+ *                  common::minimum<uint64_t>), TG_OP_MAX_U64 (MaxU64, common::maximum<uint64_t>); double with TG_OP_SUM_F64
+ *                  (std::plus<double>), TG_OP_MIN_F64 (common::minimum<double>), TG_OP_MAX_F64 (common::maximum<double>)
+ *   item_bytes 16  std::pair<uint64_t, V> with thrill_gpu::ScanSecond<F>, F any function above: .first comes from the right-hand
+ *                  operand, so the result's .first is the .first of the last worker's last item; if that worker is empty, the
+ *                  .first of what it contributes (0, or the initial value's)
+ * Anything else (TG_OP_FIRST, other item sizes) is TG_ERR_ARG.  Integer results are exact.  Min / Max on doubles are exact bit for
+ * bit: std::min(a, b) = b < a ? b : a (std::max: a < b ? b : a), so a NaN as the first operand of a fold sticks (a worker's first
+ * item, the initial value on worker 0, S_0 in the fold of the workers) and the result has that NaN's bits; a NaN anywhere else is
+ * skipped; of equal values the earliest wins (-0.0 and +0.0: the sign of a zero minimum is the earlier zero's).  The tile
+ * reduce folds positions in order with a NaN-skipping function, and the first operand goes through the stock function on its
+ * own.  Double sums are bracketed by tiles and then in a fixed order (no CTA waits on another, no atomics), so a result is
+ * bitwise reproducible from run to run.  Let exact be the exact sum of the initial value and every item, A the same sum over
+ * |x|, u = 2^-53 and gamma_D = D u / (1 - D u), where D is the longest chain of additions a summand goes through:
+ *   D = k + 31 + ceil(T / 512) + p,  k = 16 (8-byte items) or 8 (pairs),  T = the tiles of the largest worker (32 KB each)
+ * (k - 1 in a thread's run, 5 lanes, 7 warps of the tile reduce; ceil(T / 512) in a thread's run of aggregates, 5 lanes, 15 warps
+ * of the fold; 1 for the initial value; p - 1 for the workers).  D = 559 + p for 8-byte items at 2^30 - 1 items on a worker.
+ * While (1 + gamma_D) A < DBL_MAX, |out - exact| <= gamma_D A + u |exact|; NaN where the items hold a NaN or both infinities,
+ * the infinity where they hold one, and the sign of a zero (-0.0 exactly when every summand is -0.0, the T() = +0.0 of an empty
+ * worker included) are the stock fold's.  A NaN's payload is left open for sums.
+ * Limits: at most 2^30 - 1 items per worker; more on any worker is TG_ERR_TOO_LARGE on every rank (the sizes travel in the
+ * all-gather).  Collective flow: p = 1 has one host round trip (reading the value back).  With p > 1 one ncclAllGather of a
+ * 32-byte record per worker (n_local, .first, S_r) into device memory, the fold on the device, then one host read of the sizes
+ * and the value.  Inputs are read, never modified.  Collective. */
+/* on a device buffer; initial_item: item_bytes bytes on the host (NULL: none); out_item: item_bytes bytes on the host */
+int tg_all_reduce(tg_ctx* ctx, const tg_scan_desc* desc, const void* d_in, size_t n_local, const void* initial_item,
+                  void* out_item);
+/* the drop-in call (GpuAllReduceNode::Execute): a host File (Blocks) or a device File (read in place, left intact) */
+int tg_all_reduce_file(tg_ctx* ctx, const tg_scan_desc* desc, const tg_merge_input* in, const void* initial_item, void* out_item);
+/* kernel level (1 <= p <= 16 workers simulated on one device): shard w (n_shards[w] items at d_shards[w]) is worker w, which
+ * takes the initial value if w == 0.  Runs the operator's device code with each worker's record written into the slot the
+ * all-gather fills, then the fold; writes the result every rank would get.  Shards are read, never modified; a shard of 2^30 or
+ * more items is TG_ERR_TOO_LARGE. */
+int tg_all_reduce_select(tg_ctx* ctx, const tg_scan_desc* desc, const void* const* d_shards, const size_t* n_shards, uint32_t p,
+                         const void* initial_item, void* out_item);
 
 /* ---- synthetic inputs of SURVEY.md §8(d), generated on the device (bench / tests support) ------------ */
 int tg_gen_sort_uniform(tg_ctx* ctx, void* d_out, uint64_t begin, uint64_t n, uint64_t seed);

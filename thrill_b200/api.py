@@ -11,6 +11,7 @@ Mirrors (same names, argument meaning and error behaviour) the slice of thrill/a
     DIA<T>::PrefixSum / ExPrefixSum        thrill/api/dia.hpp:1850, :1867 (api/prefix_sum.hpp, ex_prefix_sum.hpp)
     DIA<T>::ZipWithIndex(zip_function)     thrill/api/zip_with_index.hpp:140-152
     api::InnerJoin(l, r, key1, key2, fn)   thrill/api/inner_join.hpp:700-827
+    DIA<T>::Sum / Min / Max / AllReduce    thrill/api/sum.hpp, min.hpp, max.hpp, all_reduce.hpp
     DIA<T>::Size / AllGather / Gather      thrill/api/size.hpp, all_gather.hpp, gather.hpp
 A DIA here holds its local shard as a host numpy array — the stand-in for a data::File whose Blocks are
 1 MiB ByteBlocks (data/byte_block.cpp:23-24, data/block_writer.hpp:405-420).  Operators hand the Blocks to the
@@ -59,9 +60,9 @@ V1_V2 = np.dtype([("v1", "<u8"), ("v2", "<u8")])                         # std::
 
 
 def ScanSecond(value_function):
-    """thrill_gpu::ScanSecond<F>: the sum function of PrefixSum on pair<uint64_t, 8-byte value>, a + b = (b.first,
-    F(a.second, b.second)), with F one of PlusU64, MinU64, MaxU64, PlusDouble"""
-    if value_function not in (PlusU64, MinU64, MaxU64, PlusDouble):
+    """thrill_gpu::ScanSecond<F>: the sum function of PrefixSum and AllReduce on pair<uint64_t, 8-byte value>, a + b = (b.first,
+    F(a.second, b.second)), with F one of PlusU64, MinU64, MaxU64, PlusDouble (and for AllReduce MinDouble, MaxDouble)"""
+    if value_function not in (PlusU64, MinU64, MaxU64, PlusDouble, MinDouble, MaxDouble):
         raise capi.ThrillGpuError("ScanSecond: %r is not a sum function the GPU path recognises" % (value_function,))
     f = _Functor("ScanSecond<%s>" % value_function.name, value_function.code)
     f.on_second = True
@@ -454,6 +455,50 @@ class DIA(object):
         return self.ReducePair(reduce_function)
 
     # ---- actions ---------------------------------------------------------------------------------------
+    def _action_desc(self, what, fn):
+        it = self.items
+        if it.ndim == 1 and it.dtype == KV:
+            if not getattr(fn, "on_second", False):
+                raise capi.ThrillGpuError("%s: pair items take ScanSecond(F) as the function" % what)
+            return capi.ScanDesc(16, fn.code)
+        if it.ndim == 1 and it.dtype == np.uint64 and fn in (PlusU64, MinU64, MaxU64):
+            return capi.ScanDesc(8, fn.code)
+        if it.ndim == 1 and it.dtype == np.float64 and fn in (PlusDouble, MinDouble, MaxDouble):
+            return capi.ScanDesc(8, fn.code)
+        raise capi.ThrillGpuError("%s: function %r on %r items is not one the GPU path recognises" % (what, fn, it.dtype))
+
+    def AllReduce(self, reduce_function, initial_value=None):
+        """DIA<T>::AllReduce(fn[, initial]) (api/all_reduce.hpp): the fold of every worker's items from its first one (worker 0
+        from initial_value, if given; an empty worker contributes T(), or initial_value if given), then of the workers' values in
+        rank order; the same value on every worker.  uint64 items with PlusU64, MinU64 or MaxU64; float64 items with PlusDouble,
+        MinDouble or MaxDouble; KV items with ScanSecond(F) (any of these F), initial_value a (first, second) tuple and the
+        result a (first, second) tuple of words"""
+        desc = self._action_desc("AllReduce", reduce_function)
+        ini = None
+        if initial_value is not None:
+            ini = np.array(initial_value, np.uint64) if desc.item_bytes == 16 else np.array([initial_value], self.items.dtype)
+        out = np.zeros(2 if desc.item_bytes == 16 else 1, np.uint64 if desc.item_bytes == 16 else self.items.dtype)
+        blocks, nb = self._blocks(self.items)
+        inp = capi.MergeInput(None, C.cast(blocks, C.POINTER(capi.Block)), nb)
+        tg = self.ctx.tg
+        tg.ck(tg.L.tg_all_reduce_file(tg.h, C.byref(desc), C.byref(inp), None if ini is None else ini.ctypes.data,
+                                      out.ctypes.data))
+        return (int(out[0]), int(out[1])) if desc.item_bytes == 16 else out[0]
+
+    def Sum(self, sum_function=None, initial_value=None):
+        """DIA<T>::Sum (api/sum.hpp): AllReduce with PlusU64 / PlusDouble by default"""
+        if sum_function is None:
+            sum_function = PlusDouble if self.items.dtype == np.float64 else PlusU64
+        return self.AllReduce(sum_function, initial_value)
+
+    def Min(self, initial_value=None):
+        """DIA<T>::Min (api/min.hpp): AllReduce with common::minimum, std::min(a, b) = b < a ? b : a"""
+        return self.AllReduce(MinDouble if self.items.dtype == np.float64 else MinU64, initial_value)
+
+    def Max(self, initial_value=None):
+        """DIA<T>::Max (api/max.hpp): AllReduce with common::maximum, std::max(a, b) = a < b ? b : a"""
+        return self.AllReduce(MaxDouble if self.items.dtype == np.float64 else MaxU64, initial_value)
+
     def Size(self):
         n = len(self.items)
         if self.ctx.num_workers() > 1:

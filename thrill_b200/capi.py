@@ -138,6 +138,9 @@ SYMBOLS = [
     ("tg_scan_local_total", _i, [_vp, _P(ScanDesc), _vp, _sz, _vp]),
     ("tg_prefix_sum_select", _i, [_vp, _P(ScanDesc), _vp, _sz, _u32, _u32, _vp, _vp, _i, _P(_vp), _P(_sz)]),
     ("tg_zip_with_index_select", _i, [_vp, _vp, _sz, _u32, _u32, _P(_u64), _i, _P(_vp), _P(_sz)]),
+    ("tg_all_reduce", _i, [_vp, _P(ScanDesc), _vp, _sz, _vp, _vp]),
+    ("tg_all_reduce_file", _i, [_vp, _P(ScanDesc), _P(MergeInput), _vp, _vp]),
+    ("tg_all_reduce_select", _i, [_vp, _P(ScanDesc), _P(_vp), _P(_sz), _u32, _vp, _vp]),
     ("tg_transfer_bytes", _i, [_vp, _P(_u64), _P(_u64)]),
     ("tg_gen_sort_uniform", _i, [_vp, _vp, _u64, _u64, _u64]),
     ("tg_gen_reduce_uniform", _i, [_vp, _vp, _u64, _u64, _u64, _u64, _i]),

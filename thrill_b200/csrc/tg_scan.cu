@@ -16,6 +16,14 @@
 // takes it from the right-hand operand, so an inclusive output keeps its item's .first and an exclusive one takes the previous
 // item's (the carry's for the worker's first item).
 // ZipWithIndex: zip_index_kernel reads 8 bytes and writes 16 per item; the base index is the sum of the lower ranks' sizes.
+//
+// The actions Sum / Min / Max / AllReduce (AllReduceNode, api/all_reduce.hpp:27-85) reuse the tile reduce and the record:
+//   1. scan_reduce_kernel   one aggregate per tile (8 bytes per item read, 16 for pairs, nothing written but the aggregates)
+//   2. action_fold_kernel   one CTA: phase TOTAL folds the aggregates in order into the worker's value and writes its record;
+//                           phase RESULT folds the p records (all-gathered, or filled in place by _select) in rank order
+// Min / Max on doubles are exact and not commutative (std::min(a, b) = b < a ? b : a keeps the earlier of two equal values, and
+// a NaN first operand sticks).  Their tile reduce folds positions in order (each thread a contiguous run, then lanes and warps
+// in order) with a NaN-skipping function, and the first operand of the stock fold is applied on its own in the fold kernel.
 #include "tg_common.cuh"
 
 namespace {
@@ -31,24 +39,44 @@ constexpr int ST_THREADS = 512;                 // scan_prefix_kernel (one CTA)
 constexpr int ST_PER = 8;                       // aggregates per thread and round
 constexpr int ZIP_THREADS = 256, ZIP_PER = 4;
 
-enum { STEP_REDUCE = 1, STEP_TOTAL = 2, STEP_PREFIX = 4, STEP_SCAN = 8 };
+enum { STEP_REDUCE = 1, STEP_TOTAL = 2, STEP_PREFIX = 4, STEP_SCAN = 8, STEP_RESULT = 16 };
 
 // what each worker contributes to the all-gather: its size and its local total S (for pairs: S.first = the .first of its
 // last item, 0 if it has none)
 struct ScanRec { u64 n, first, value, pad; };
 
-// the one combine function of the sum functions on the 8-byte value, used by every kernel and by the carry fold
+// Min / Max on doubles: partial folds must keep positions in order
+template <int OP>
+__host__ __device__ constexpr bool in_order() { return OP == TG_OP_MIN_F64 || OP == TG_OP_MAX_F64; }
+
+// the one combine function of the sum functions on the 8-byte value, used by every kernel and by the carry fold.  For Min / Max
+// on doubles it skips a NaN operand (a NaN is its identity) and keeps the left operand of two equal values; the stock function,
+// whose NaN first operand sticks, is stock_fn.
 template <int OP>
 __device__ __forceinline__ u64 combine(u64 a, u64 b) {
     if (OP == TG_OP_SUM_F64) return (u64)__double_as_longlong(__longlong_as_double((long long)a) + __longlong_as_double((long long)b));
     if (OP == TG_OP_SUM_U64) return a + b;
     if (OP == TG_OP_MIN_U64) return b < a ? b : a;
+    if (in_order<OP>()) {
+        const double x = __longlong_as_double((long long)a), y = __longlong_as_double((long long)b);
+        if (x != x) return b;
+        return (OP == TG_OP_MIN_F64 ? y < x : x < y) ? b : a;
+    }
     return a < b ? b : a;                       // TG_OP_MAX_U64
 }
-// the exact identity of the partial folds (-0.0 for double sums: x + -0.0 == x for every x, including -0.0)
+// the stock function: common::minimum / maximum (std::min / std::max) on doubles, combine otherwise
+template <int OP>
+__device__ __forceinline__ u64 stock_fn(u64 a, u64 b) {
+    if (!in_order<OP>()) return combine<OP>(a, b);
+    const double x = __longlong_as_double((long long)a), y = __longlong_as_double((long long)b);
+    return (OP == TG_OP_MIN_F64 ? y < x : x < y) ? b : a;
+}
+// the exact identity of the partial folds (-0.0 for double sums: x + -0.0 == x for every x, including -0.0; a quiet NaN for
+// Min / Max on doubles)
 template <int OP>
 __device__ __forceinline__ u64 ident() {
-    return OP == TG_OP_SUM_F64 ? 0x8000000000000000ull : OP == TG_OP_MIN_U64 ? ~0ull : 0ull;
+    return OP == TG_OP_SUM_F64 ? 0x8000000000000000ull : OP == TG_OP_MIN_U64 ? ~0ull
+         : in_order<OP>() ? 0x7ff8000000000000ull : 0ull;
 }
 // T(): the value-initialised item the stock node folds its local total from (+0.0, 0)
 constexpr u64 T_VALUE = 0;
@@ -67,6 +95,13 @@ __device__ __forceinline__ u64 warp_reduce(u64 v) {
     for (int d = 16; d >= 1; d >>= 1) v = combine<OP>(v, __shfl_down_sync(0xffffffffu, v, d));
     return v;                                   // (lane 0)
 }
+// the same with lane 0 holding the lanes' values folded in lane order
+template <int OP>
+__device__ __forceinline__ u64 warp_reduce_in_order(u64 v) {
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) v = combine<OP>(v, __shfl_down_sync(0xffffffffu, v, d));
+    return v;                                   // (lane 0)
+}
 
 // inclusive scan over the lanes (left to right), and the exclusive value of each lane
 template <int OP>
@@ -82,18 +117,19 @@ __device__ __forceinline__ u64 warp_scan(u64 v, u64* excl) {
     return v;
 }
 
-// pass 1: agg[tile] = the fold of the tile's values
+// pass 1: agg[tile] = the fold of the tile's values (in position order for in_order ops: thread t takes the units 8t..8t+7)
 template <int OP, int IB>
 __global__ void __launch_bounds__(SC_THREADS) scan_reduce_kernel(const ulonglong2* __restrict__ in, u64 n, u64* __restrict__ agg) {
     __shared__ u64 wsum[SC_THREADS / 32];
-    const u64 ubase = (u64)blockIdx.x * TILE_UNITS + threadIdx.x;
+    const u64 tile = (u64)blockIdx.x * TILE_UNITS;
     ulonglong2 v[SC_UNITS];
 #pragma unroll
-    for (int j = 0; j < SC_UNITS; ++j) v[j] = load_unit<OP, IB>(in, ubase + (u64)j * SC_THREADS, n);
+    for (int j = 0; j < SC_UNITS; ++j)
+        v[j] = load_unit<OP, IB>(in, in_order<OP>() ? tile + threadIdx.x * SC_UNITS + j : tile + threadIdx.x + (u64)j * SC_THREADS, n);
     u64 acc = IB == 16 ? v[0].y : combine<OP>(v[0].x, v[0].y);
 #pragma unroll
     for (int j = 1; j < SC_UNITS; ++j) acc = IB == 16 ? combine<OP>(acc, v[j].y) : combine<OP>(combine<OP>(acc, v[j].x), v[j].y);
-    acc = warp_reduce<OP>(acc);
+    acc = in_order<OP>() ? warp_reduce_in_order<OP>(acc) : warp_reduce<OP>(acc);
     if (lane_id() == 0) wsum[threadIdx.x / 32] = acc;
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -249,6 +285,50 @@ __global__ void __launch_bounds__(ZIP_THREADS) zip_index_kernel(const u64* __res
     }
 }
 
+// The actions.  Phase TOTAL: R = agg_0 + ... + agg_{ntiles-1} in order (each thread a contiguous run, then lanes and warps in
+// order), and *my_rec = (n, .first of the last item, W) with the stock node's worker value (all_reduce.hpp:36-63, whose value
+// starts as the initial value on every worker):
+//   no items: the initial value if there is one (init & INIT_GIVEN), else T();  otherwise initial + R on the worker that folds
+//   it (init & INIT_FOLD: worker 0), else R (the fold of every item from the first).  For Min / Max on doubles the first
+//   operand, initial or x_0, goes through the stock function.
+// Phase RESULT: out = (recs[p-1].first, recs[0] + ... + recs[p-1]) folded left to right with the stock function.
+enum { INIT_GIVEN = 1, INIT_FOLD = 2 };
+template <int OP, int IB>
+__global__ void __launch_bounds__(ST_THREADS) action_fold_kernel(const u64* __restrict__ agg, u32 ntiles, u32 steps,
+                                                                 const ulonglong2* __restrict__ in, u64 n, int init,
+                                                                 u64 init_first, u64 init_value, ScanRec* my_rec,
+                                                                 const ScanRec* recs, u32 p, u64* out) {
+    __shared__ u64 wsum[ST_THREADS / 32];
+    const u32 tid = threadIdx.x;
+    if (steps & STEP_TOTAL) {
+        const u32 per = (ntiles + ST_THREADS - 1) / ST_THREADS, b = tid * per, e = min(b + per, ntiles);
+        u64 acc = ident<OP>();
+        for (u32 i = b; i < e; ++i) acc = combine<OP>(acc, agg[i]);
+        acc = warp_reduce_in_order<OP>(acc);
+        if (lane_id() == 0) wsum[tid / 32] = acc;
+        __syncthreads();
+        if (tid == 0) {
+            u64 r = wsum[0];
+            for (int w = 1; w < ST_THREADS / 32; ++w) r = combine<OP>(r, wsum[w]);
+            u64 first = 0, value = T_VALUE;
+            const bool fold_init = init & INIT_FOLD;
+            if (n) {
+                first = IB == 16 ? in[n - 1].x : 0;
+                if (in_order<OP>()) value = stock_fn<OP>(fold_init ? init_value : IB == 16 ? in[0].y : in[0].x, r);
+                else value = fold_init ? combine<OP>(init_value, r) : r;
+            }
+            else if (init & INIT_GIVEN) { first = init_first; value = init_value; }
+            *my_rec = ScanRec{ n, first, value, 0 };
+        }
+    }
+    if ((steps & STEP_RESULT) && tid == 0) {
+        u64 v = recs[0].value;
+        for (u32 r = 1; r < p; ++r) v = stock_fn<OP>(v, recs[r].value);
+        out[0] = recs[p - 1].first;
+        out[1] = v;
+    }
+}
+
 // ---- host side ---------------------------------------------------------------------------------------------------------------
 
 // one scan on one worker.  The WS_SCAN_AUX workspace holds, in this order: carry (2 words), this worker's record, the p
@@ -315,13 +395,20 @@ int check_desc(tg_ctx* ctx, const tg_scan_desc* desc) {
     return TG_OK;
 }
 
-// the job's workspaces: aux (records, aggregates, prefixes) and the output of n_out items of out_bytes
-int prepare(tg_ctx* ctx, ScanJob* j, uint32_t out_bytes) {
-    const u64 n = j->n < SCAN_LIMIT ? j->n : 0;         // (an input over the limit is only counted, never read)
+// the job's aux workspace (records, aggregates, prefixes) for n items
+int prepare_aux(tg_ctx* ctx, ScanJob* j, u64 n) {
+    n = n < SCAN_LIMIT ? n : 0;                         // (an input over the limit is only counted, never read)
     const u64 nt = (n * j->ib + TILE_UNITS * 16 - 1) / (TILE_UNITS * 16);
     void* aux;
     TG_TRY(tg_ws_get(ctx, WS_SCAN_AUX, AUX_TILES + (nt + 2) * 16, &aux));
     j->aux = (char*)aux;
+    return TG_OK;
+}
+
+// ... and the output of n items of out_bytes
+int prepare(tg_ctx* ctx, ScanJob* j, uint32_t out_bytes) {
+    const u64 n = j->n < SCAN_LIMIT ? j->n : 0;
+    TG_TRY(prepare_aux(ctx, j, j->n));
     void* out;
     TG_TRY(tg_ws_get(ctx, WS_SCAN_OUT, n * out_bytes + 16, &out));
     j->out = out;
@@ -435,6 +522,91 @@ int stage_input(tg_ctx* ctx, const tg_merge_input* in, uint32_t item_bytes, cons
     return TG_OK;
 }
 
+// ---- the actions ------------------------------------------------------------------------------------------------------------
+
+int check_action_desc(tg_ctx* ctx, const tg_scan_desc* desc) {
+    if (!desc) return tg_set_error(ctx, TG_ERR_ARG, "all_reduce: NULL descriptor");
+    if (desc->item_bytes != 8 && desc->item_bytes != 16)
+        return tg_set_error(ctx, TG_ERR_ARG, "all_reduce: %u-byte items (8: uint64_t / double, 16: pair<uint64_t, V>)", desc->item_bytes);
+    if (desc->op > TG_OP_MAX_F64)
+        return tg_set_error(ctx, TG_ERR_ARG, "all_reduce: op %u (sum, min and max of uint64_t and double only)", desc->op);
+    return TG_OK;
+}
+
+// steps of one worker (STEP_REDUCE | STEP_TOTAL into *rec) and / or the fold of the p records at j.recs() (STEP_RESULT into
+// j.carry()); init: INIT_GIVEN | INIT_FOLD flags of this worker
+template <int OP, int IB>
+int action_steps(tg_ctx* ctx, const ScanJob& j, int steps, int init, ScanRec* rec, u32 p) {
+    const u32 nt = j.ntiles();
+    const ulonglong2* in = (const ulonglong2*)j.in;
+    if ((steps & STEP_REDUCE) && nt)
+        TG_LAUNCH_T(ctx, TG_K_SCAN, (scan_reduce_kernel<OP, IB>), nt, SC_THREADS, 0, in, j.n, j.agg());
+    if (steps & (STEP_TOTAL | STEP_RESULT))
+        TG_LAUNCH_T(ctx, TG_K_SCAN, (action_fold_kernel<OP, IB>), 1, ST_THREADS, 0, (const u64*)j.agg(), nt,
+                    (u32)(steps & (STEP_TOTAL | STEP_RESULT)), in, j.n, init, j.init_first, j.init_value, rec,
+                    (const ScanRec*)j.recs(), p, j.carry());
+    return TG_OK;
+}
+
+template <int OP>
+int action_steps_ib(tg_ctx* ctx, const ScanJob& j, int steps, int init, ScanRec* rec, u32 p) {
+    return j.ib == 16 ? action_steps<OP, 16>(ctx, j, steps, init, rec, p) : action_steps<OP, 8>(ctx, j, steps, init, rec, p);
+}
+
+int action_run(tg_ctx* ctx, const ScanJob& j, int steps, int init, ScanRec* rec, u32 p) {
+    switch (j.op) {
+    case TG_OP_SUM_F64: return action_steps_ib<TG_OP_SUM_F64>(ctx, j, steps, init, rec, p);
+    case TG_OP_SUM_U64: return action_steps_ib<TG_OP_SUM_U64>(ctx, j, steps, init, rec, p);
+    case TG_OP_MIN_U64: return action_steps_ib<TG_OP_MIN_U64>(ctx, j, steps, init, rec, p);
+    case TG_OP_MAX_U64: return action_steps_ib<TG_OP_MAX_U64>(ctx, j, steps, init, rec, p);
+    case TG_OP_MIN_F64: return action_steps_ib<TG_OP_MIN_F64>(ctx, j, steps, init, rec, p);
+    default: return action_steps_ib<TG_OP_MAX_F64>(ctx, j, steps, init, rec, p);
+    }
+}
+
+// the one host read: the result words and the p records (aux bytes [0, AUX_RECS + p records)), then the verdict on the limit
+// (the same on every rank) and the result item
+int action_finish(tg_ctx* ctx, const ScanJob& j, u32 p, const char* what, void* out_item) {
+    char* h = (char*)ctx->pinned;
+    TG_CUDA(ctx, cudaMemcpyAsync(h, j.aux, AUX_RECS + p * sizeof(ScanRec), cudaMemcpyDeviceToHost, ctx->stream));
+    TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    const ScanRec* recs = (const ScanRec*)(h + AUX_RECS);
+    for (u32 r = 0; r < p; ++r)
+        if (recs[r].n >= SCAN_LIMIT)
+            return tg_set_error(ctx, TG_ERR_TOO_LARGE, "%s: worker %u holds %llu items (limit 2^30 - 1)", what, r,
+                                (unsigned long long)recs[r].n);
+    const u64* res = (const u64*)(h + AUX_CARRY);
+    if (j.ib == 16) memcpy(out_item, res, 16);
+    else memcpy(out_item, &res[1], 8);
+    return TG_OK;
+}
+
+// p = 1: the reduce and both fold phases, one host read.  p > 1: this worker's record (written from the host if it is over the
+// limit: only its size is read), one ncclAllGather of the records into device memory, the fold, one host read.
+int all_reduce_impl(tg_ctx* ctx, const tg_scan_desc* desc, const void* d_in, size_t n_local, const void* initial_item,
+                    void* out_item) {
+    const int p = ctx->nranks;
+    if (p == 1 && n_local >= SCAN_LIMIT)
+        return tg_set_error(ctx, TG_ERR_TOO_LARGE, "all_reduce: n_local=%zu (limit 2^30 - 1)", n_local);
+    ScanJob j;
+    j.op = desc->op; j.ib = desc->item_bytes; j.in = d_in; j.n = n_local; j.rank = (u32)ctx->rank;
+    set_initial(&j, initial_item);
+    const int init = initial_item ? INIT_GIVEN | (ctx->rank == 0 ? INIT_FOLD : 0) : 0;
+    TG_TRY(prepare_aux(ctx, &j, j.n));
+    if (p == 1) TG_TRY(action_run(ctx, j, STEP_REDUCE | STEP_TOTAL | STEP_RESULT, init, j.recs(), 1));
+    else {
+        if (n_local < SCAN_LIMIT) TG_TRY(action_run(ctx, j, STEP_REDUCE | STEP_TOTAL, init, j.my_rec(), p));
+        else {
+            ScanRec* hr = (ScanRec*)ctx->pinned;
+            *hr = ScanRec{ j.n, 0, 0, 0 };
+            TG_CUDA(ctx, cudaMemcpyAsync(j.my_rec(), hr, sizeof(ScanRec), cudaMemcpyHostToDevice, ctx->stream));
+        }
+        TG_NCCL(ctx, ncclAllGather(j.my_rec(), j.recs(), sizeof(ScanRec) / 8, ncclUint64, ctx->comm, ctx->stream));
+        TG_TRY(action_run(ctx, j, STEP_RESULT, 0, nullptr, p));
+    }
+    return action_finish(ctx, j, p, "all_reduce", out_item);
+}
+
 }  // namespace
 
 extern "C" {
@@ -543,6 +715,53 @@ int tg_zip_with_index_select(tg_ctx* ctx, const void* d_in, size_t n_local, uint
     *out_dptr = j.out;
     *out_n = n_local;
     return TG_OK;
+}
+
+int tg_all_reduce(tg_ctx* ctx, const tg_scan_desc* desc, const void* d_in, size_t n_local, const void* initial_item,
+                  void* out_item) {
+    if (!ctx || !out_item || (!d_in && n_local)) return tg_set_error(ctx, TG_ERR_ARG, "all_reduce: NULL argument");
+    TG_TRY(check_action_desc(ctx, desc));
+    TG_TRY(check_ranks(ctx));
+    TG_CUDA(ctx, cudaSetDevice(ctx->device));
+    return all_reduce_impl(ctx, desc, d_in, n_local, initial_item, out_item);
+}
+
+int tg_all_reduce_file(tg_ctx* ctx, const tg_scan_desc* desc, const tg_merge_input* in, const void* initial_item, void* out_item) {
+    if (!ctx || !in || !out_item) return tg_set_error(ctx, TG_ERR_ARG, "all_reduce_file: NULL argument");
+    TG_TRY(check_action_desc(ctx, desc));
+    TG_TRY(check_ranks(ctx));
+    TG_CUDA(ctx, cudaSetDevice(ctx->device));
+    const void* d_in;
+    size_t n;
+    TG_TRY(stage_input(ctx, in, desc->item_bytes, &d_in, &n));
+    return all_reduce_impl(ctx, desc, d_in, n, initial_item, out_item);
+}
+
+int tg_all_reduce_select(tg_ctx* ctx, const tg_scan_desc* desc, const void* const* d_shards, const size_t* n_shards, uint32_t p,
+                         const void* initial_item, void* out_item) {
+    if (!ctx || !d_shards || !n_shards || !out_item || p == 0 || p > TG_MAX_RANKS)
+        return tg_set_error(ctx, TG_ERR_ARG, "all_reduce_select: p=%u or a NULL argument", p);
+    TG_TRY(check_action_desc(ctx, desc));
+    u64 largest = 0;
+    for (uint32_t w = 0; w < p; ++w) {
+        if (!d_shards[w] && n_shards[w]) return tg_set_error(ctx, TG_ERR_ARG, "all_reduce_select: shard %u is NULL", w);
+        if (n_shards[w] >= SCAN_LIMIT)
+            return tg_set_error(ctx, TG_ERR_TOO_LARGE, "all_reduce_select: shard %u holds %zu items (limit 2^30 - 1)", w, n_shards[w]);
+        largest = n_shards[w] > largest ? n_shards[w] : largest;
+    }
+    TG_CUDA(ctx, cudaSetDevice(ctx->device));
+    ScanJob j;
+    j.op = desc->op; j.ib = desc->item_bytes;
+    set_initial(&j, initial_item);
+    TG_TRY(prepare_aux(ctx, &j, largest));
+    // worker w's record into the slot the all-gather fills
+    for (uint32_t w = 0; w < p; ++w) {
+        j.in = d_shards[w]; j.n = n_shards[w]; j.rank = w;
+        TG_TRY(action_run(ctx, j, STEP_REDUCE | STEP_TOTAL, initial_item ? INIT_GIVEN | (w == 0 ? INIT_FOLD : 0) : 0,
+                          j.recs() + w, p));
+    }
+    TG_TRY(action_run(ctx, j, STEP_RESULT, 0, nullptr, p));
+    return action_finish(ctx, j, p, "all_reduce_select", out_item);
 }
 
 }  // extern "C"

@@ -11,6 +11,8 @@
  *     thrill_gpu::GroupToIndex<Out>(dia, KeyFirst(), fn, size)    <->  DIA<T>::GroupToIndex (api/group_to_index.hpp:257)
  *     thrill_gpu::PrefixSum(dia, fn [, initial]) / ExPrefixSum    <->  DIA<T>::PrefixSum / ExPrefixSum (api/dia.hpp:1850, :1867)
  *     thrill_gpu::ZipWithIndex(dia, IndexFirst() | IndexSecond()) <->  DIA<T>::ZipWithIndex (api/zip_with_index.hpp:140)
+ *     thrill_gpu::Sum / Min / Max / AllReduce (dia, ...) [Future]  <->  DIA<T>::Sum / Min / Max / AllReduce (api/sum.hpp, ...)
+ *     thrill_gpu::Size(dia) / SizeFuture(dia)                     <->  DIA<T>::Size / SizeFuture (api/size.hpp)
  * Everything else of the pipeline (sources, LOps, other DOps, actions, the net/data layers) is the
  * UNMODIFIED reference library: this header only includes it.  The heavy lifting happens behind the C ABI
  * of include/thrill_gpu.h (libthrill_gpu.so): the nodes hand the Blocks of their input data::File to
@@ -29,9 +31,11 @@
 #ifndef THRILL_GPU_NODES_HEADER
 #define THRILL_GPU_NODES_HEADER
 
+#include <thrill/api/action_node.hpp>
 #include <thrill/api/dia.hpp>
 #include <thrill/api/dop_node.hpp>
 #include <thrill/common/config.hpp>
+#include <thrill/common/functional.hpp>
 #include <thrill/data/file.hpp>
 #include <tlx/meta/call_foreach_with_index.hpp>
 #include <tlx/meta/vexpand.hpp>
@@ -232,7 +236,7 @@ struct JoinDesc<JoinValues>{
 //! operator() (the stock nodes read its argument type), so the stock DIA::PrefixSum takes it too.
 template <typename MemberFn> struct MemberResult;
 template <typename R, typename C, typename... A>
-struct MemberResult<R (C::*)(A...) const> { using type = R; };
+struct MemberResult<R (C::*)(A...) const> { using type = typename std::decay<R>::type; };   // (common::minimum returns const T&)
 template <typename ValueFunction>
 struct ScanSecond {
     using Pair = std::pair<uint64_t, typename MemberResult<decltype(&ValueFunction::operator ())>::type>;
@@ -253,6 +257,27 @@ struct ScanDesc : ScanOp<ValueType, SumFunction> { static constexpr uint32_t ite
 template <typename V, typename F>
 struct ScanDesc<std::pair<uint64_t, V>, ScanSecond<F> >
     : ScanOp<typename std::conditional<std::is_same<V, typename ScanSecond<F>::Pair::second_type>::value, V, void>::type, F>{
+    static constexpr uint32_t item_bytes = 16;
+};
+//! the (item type, function) pairs of Sum / Min / Max / AllReduce: those of PrefixSum, and common::minimum / common::maximum
+//! (what the stock Min / Max use) on uint64_t and double, also inside ScanSecond<F> on pairs
+template <typename Value, typename Function>
+struct ActionOp : ScanOp<Value, Function> { };
+template <uint32_t kOp>
+struct ActionOpIs { static constexpr bool supported = true; static constexpr uint32_t op = kOp; };
+template <>
+struct ActionOp<uint64_t, thrill::common::minimum<uint64_t> >: ActionOpIs<TG_OP_MIN_U64> { };
+template <>
+struct ActionOp<uint64_t, thrill::common::maximum<uint64_t> >: ActionOpIs<TG_OP_MAX_U64> { };
+template <>
+struct ActionOp<double, thrill::common::minimum<double> >: ActionOpIs<TG_OP_MIN_F64> { };
+template <>
+struct ActionOp<double, thrill::common::maximum<double> >: ActionOpIs<TG_OP_MAX_F64> { };
+template <typename ValueType, typename Function>
+struct ActionDesc : ActionOp<ValueType, Function> { static constexpr uint32_t item_bytes = 8; };
+template <typename V, typename F>
+struct ActionDesc<std::pair<uint64_t, V>, ScanSecond<F> >
+    : ActionOp<typename std::conditional<std::is_same<V, typename ScanSecond<F>::Pair::second_type>::value, V, void>::type, F>{
     static constexpr uint32_t item_bytes = 16;
 };
 //! The zip functions thrill_gpu::ZipWithIndex recognises on 8-byte items: (item, index) -> pair(index, item) or pair(item, index)
@@ -1032,6 +1057,115 @@ using GpuPrefixSumNode = GpuScanNode<ValueType, ValueType>;
 template <typename ValueOut, typename ValueIn>
 using GpuZipWithIndexNode = GpuScanNode<ValueOut, ValueIn>;
 
+//! DIA::Sum / Min / Max / AllReduce (AllReduceNode, api/all_reduce.hpp:27-85): the stock node protocol (a File of the parent's
+//! items, or the parent's File whole through OnPreOpFile) with the collective call in Execute: tg_all_reduce_file (the tile
+//! reduce, one all-gather of the workers' records, the fold on the device).  A parent GPU node hands its result over in HBM, so
+//! a GPU chain that ends in an action fetches nothing but the value.  The result is the stock node's bit for bit, except for the
+//! bracketing of double sums (include/thrill_gpu.h states the bound).
+template <typename ValueType>
+class GpuAllReduceNode final : public thrill::api::ActionResultNode<ValueType>, public GpuNodeBase
+{
+    using Super = thrill::api::ActionResultNode<ValueType>;
+    using Super::context_;
+
+public:
+    template <typename ParentDIA>
+    GpuAllReduceNode(const ParentDIA& parent, const char* label, const tg_scan_desc& desc, const ValueType& initial,
+                     bool with_initial)
+        : Super(parent.ctx(), label, { parent.id() }, { parent.node() }),
+          desc_(desc), initial_(initial), with_initial_(with_initial), parent_stack_empty_(ParentDIA::stack_empty) {
+        auto pre_op_fn = [this](const ValueType& input) { input_writer_.Put(input); };
+        auto lop_chain = parent.stack().push(pre_op_fn).fold();
+        parent.node()->AddChild(this, lop_chain);
+    }
+
+    void StartPreOp(size_t /* parent_index */) final { input_writer_ = input_file_.GetWriter(); }
+
+    bool OnPreOpFile(const thrill::data::File& file, size_t /* parent_index */) final {
+        if (!parent_stack_empty_) return false;
+        input_file_ = file.Copy();
+        return true;
+    }
+
+    bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes, size_t /* parent_index */) final {
+        if (!parent_stack_empty_ || item_bytes != sizeof(ValueType)) return false;
+        device_input_ = file;
+        return true;
+    }
+
+    void StopPreOp(size_t /* parent_index */) final { input_writer_.Close(); }
+
+    //! Execute (all_reduce.hpp:67-70) behind one call.  Collective.
+    void Execute() final {
+        tg_ctx* c = WorkerCtx(context_);
+        std::unique_ptr<PinnedFileView> view;
+        tg_merge_input in;
+        if (device_input_) {
+            in = tg_merge_input { device_input_->get(), nullptr, 0 };
+        }
+        else {
+            view.reset(new PinnedFileView(input_file_, context_.local_worker_id()));
+            in = tg_merge_input { nullptr, view->data(), view->size() };
+        }
+        Check(c, tg_all_reduce_file(c, &desc_, &in, with_initial_ ? &initial_ : nullptr, &result_), "tg_all_reduce_file");
+        view.reset();
+        input_file_.Clear();
+        device_input_.reset();
+    }
+
+    const ValueType& result() const final { return result_; }
+
+private:
+    const tg_scan_desc desc_;
+    const ValueType initial_;
+    const bool with_initial_;
+    const bool parent_stack_empty_;
+    thrill::data::File input_file_ { context_.GetFile(this) };
+    thrill::data::File::Writer input_writer_;
+    DeviceFilePtr device_input_;
+    ValueType result_ = ValueType();
+};
+
+//! DIA::Size / SizeFuture (SizeNode, api/size.hpp): the local count from a device File's items(), a host File's num_items() or
+//! the per-item PreOp, then the stock all-reduce of the counts.  No kernel, and no item crosses PCIe.
+template <typename ValueType>
+class GpuSizeNode final : public thrill::api::ActionResultNode<size_t>, public GpuNodeBase
+{
+    using Super = thrill::api::ActionResultNode<size_t>;
+    using Super::context_;
+
+public:
+    template <typename ParentDIA>
+    explicit GpuSizeNode(const ParentDIA& parent)
+        : Super(parent.ctx(), "GpuSize", { parent.id() }, { parent.node() }),
+          parent_stack_empty_(ParentDIA::stack_empty) {
+        auto pre_op_fn = [this](const ValueType&) { ++local_size_; };
+        auto lop_chain = parent.stack().push(pre_op_fn).fold();
+        parent.node()->AddChild(this, lop_chain);
+    }
+
+    bool OnPreOpFile(const thrill::data::File& file, size_t /* parent_index */) final {
+        if (!parent_stack_empty_) return false;
+        local_size_ = file.num_items();
+        return true;
+    }
+
+    bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes, size_t /* parent_index */) final {
+        if (!parent_stack_empty_ || item_bytes != sizeof(ValueType)) return false;
+        local_size_ = file->items();
+        return true;
+    }
+
+    void Execute() final { global_size_ = context_.net.AllReduce(local_size_); }
+
+    const size_t& result() const final { return global_size_; }
+
+private:
+    const bool parent_stack_empty_;
+    size_t local_size_ = 0;
+    size_t global_size_ = 0;
+};
+
 /******************************************************************************/
 // front doors (same argument meaning as DIA<T>::Sort / DIA<T>::ReducePair)
 
@@ -1239,6 +1373,105 @@ auto ZipWithIndex(const DIA<ValueType, Stack>& dia, const ZipFunction& zip_funct
         std::is_same<ZipFunction, IndexFirst>::value);
     return DIA<ValueOut>(node);
 }
+
+//! DIA<T>::AllReduceFuture(fn[, initial]) (api/all_reduce.hpp:157-221) for the recognised pairs: uint64_t with std::plus<uint64_t>,
+//! MinU64 / common::minimum<uint64_t> or MaxU64 / common::maximum<uint64_t>; double with std::plus<double>,
+//! common::minimum<double> or common::maximum<double>; pair<uint64_t, V> with ScanSecond<F>, F any of these.  Each worker folds
+//! its items from its first one (worker 0 from initial), an empty worker contributes T() (the initial value if there is one),
+//! and the workers' values are folded in rank order: the stock result, bit for bit, but for the bracketing of double sums
+//! (bitwise reproducible, within the bound of tg_all_reduce in include/thrill_gpu.h).
+template <typename ValueType, typename Stack, typename Function>
+thrill::api::Future<ValueType> AllReduceFuture(const DIA<ValueType, Stack>& dia, const Function& /* function */) {
+    static_assert(ActionDesc<ValueType, Function>::supported,
+                  "thrill_gpu::AllReduce: this (ValueType, Function) pair has no GPU descriptor; use the stock dia.AllReduce(fn)");
+    assert(dia.IsValid());
+    auto node = tlx::make_counting<GpuAllReduceNode<ValueType> >(
+        dia, "GpuAllReduce", tg_scan_desc { ActionDesc<ValueType, Function>::item_bytes, ActionDesc<ValueType, Function>::op },
+        ValueType(), false);
+    return thrill::api::Future<ValueType>(node);
+}
+template <typename ValueType, typename Stack, typename Function>
+thrill::api::Future<ValueType> AllReduceFuture(const DIA<ValueType, Stack>& dia, const Function& /* function */,
+                                               const typename DIA<ValueType, Stack>::ValueType& initial_value) {
+    static_assert(ActionDesc<ValueType, Function>::supported,
+                  "thrill_gpu::AllReduce: this (ValueType, Function) pair has no GPU descriptor; use the stock dia.AllReduce(fn)");
+    assert(dia.IsValid());
+    auto node = tlx::make_counting<GpuAllReduceNode<ValueType> >(
+        dia, "GpuAllReduce", tg_scan_desc { ActionDesc<ValueType, Function>::item_bytes, ActionDesc<ValueType, Function>::op },
+        initial_value, true);
+    return thrill::api::Future<ValueType>(node);
+}
+//! DIA<T>::AllReduce(fn[, initial]) (api/all_reduce.hpp:87-155)
+template <typename ValueType, typename Stack, typename Function>
+ValueType AllReduce(const DIA<ValueType, Stack>& dia, const Function& function) {
+    return AllReduceFuture(dia, function).get();
+}
+template <typename ValueType, typename Stack, typename Function>
+ValueType AllReduce(const DIA<ValueType, Stack>& dia, const Function& function,
+                    const typename DIA<ValueType, Stack>::ValueType& initial_value) {
+    return AllReduceFuture(dia, function, initial_value).get();
+}
+//! DIA<T>::Sum / SumFuture([fn[, initial]]) (api/sum.hpp): AllReduce with std::plus<T> by default
+template <typename ValueType, typename Stack, typename SumFunction = std::plus<ValueType> >
+thrill::api::Future<ValueType> SumFuture(const DIA<ValueType, Stack>& dia, const SumFunction& sum_function = SumFunction()) {
+    return AllReduceFuture(dia, sum_function);
+}
+template <typename ValueType, typename Stack, typename SumFunction>
+thrill::api::Future<ValueType> SumFuture(const DIA<ValueType, Stack>& dia, const SumFunction& sum_function,
+                                         const typename DIA<ValueType, Stack>::ValueType& initial_value) {
+    return AllReduceFuture(dia, sum_function, initial_value);
+}
+template <typename ValueType, typename Stack, typename SumFunction = std::plus<ValueType> >
+ValueType Sum(const DIA<ValueType, Stack>& dia, const SumFunction& sum_function = SumFunction()) {
+    return SumFuture(dia, sum_function).get();
+}
+template <typename ValueType, typename Stack, typename SumFunction>
+ValueType Sum(const DIA<ValueType, Stack>& dia, const SumFunction& sum_function,
+              const typename DIA<ValueType, Stack>::ValueType& initial_value) {
+    return SumFuture(dia, sum_function, initial_value).get();
+}
+//! DIA<T>::Min / MinFuture([initial]) (api/min.hpp): AllReduce with common::minimum<T> (std::min: b < a ? b : a)
+template <typename ValueType, typename Stack>
+thrill::api::Future<ValueType> MinFuture(const DIA<ValueType, Stack>& dia) {
+    return AllReduceFuture(dia, thrill::common::minimum<ValueType>());
+}
+template <typename ValueType, typename Stack>
+thrill::api::Future<ValueType> MinFuture(const DIA<ValueType, Stack>& dia,
+                                         const typename DIA<ValueType, Stack>::ValueType& initial_value) {
+    return AllReduceFuture(dia, thrill::common::minimum<ValueType>(), initial_value);
+}
+template <typename ValueType, typename Stack>
+ValueType Min(const DIA<ValueType, Stack>& dia) { return MinFuture(dia).get(); }
+template <typename ValueType, typename Stack>
+ValueType Min(const DIA<ValueType, Stack>& dia, const typename DIA<ValueType, Stack>::ValueType& initial_value) {
+    return MinFuture(dia, initial_value).get();
+}
+//! DIA<T>::Max / MaxFuture([initial]) (api/max.hpp): AllReduce with common::maximum<T> (std::max: a < b ? b : a)
+template <typename ValueType, typename Stack>
+thrill::api::Future<ValueType> MaxFuture(const DIA<ValueType, Stack>& dia) {
+    return AllReduceFuture(dia, thrill::common::maximum<ValueType>());
+}
+template <typename ValueType, typename Stack>
+thrill::api::Future<ValueType> MaxFuture(const DIA<ValueType, Stack>& dia,
+                                         const typename DIA<ValueType, Stack>::ValueType& initial_value) {
+    return AllReduceFuture(dia, thrill::common::maximum<ValueType>(), initial_value);
+}
+template <typename ValueType, typename Stack>
+ValueType Max(const DIA<ValueType, Stack>& dia) { return MaxFuture(dia).get(); }
+template <typename ValueType, typename Stack>
+ValueType Max(const DIA<ValueType, Stack>& dia, const typename DIA<ValueType, Stack>::ValueType& initial_value) {
+    return MaxFuture(dia, initial_value).get();
+}
+
+//! DIA<T>::SizeFuture / Size (api/size.hpp:86-103): the number of items of the DIA, on every worker.  Any item type.
+template <typename ValueType, typename Stack>
+thrill::api::Future<size_t> SizeFuture(const DIA<ValueType, Stack>& dia) {
+    assert(dia.IsValid());
+    auto node = tlx::make_counting<GpuSizeNode<ValueType> >(dia);
+    return thrill::api::Future<size_t>(node);
+}
+template <typename ValueType, typename Stack>
+size_t Size(const DIA<ValueType, Stack>& dia) { return SizeFuture(dia).get(); }
 
 } // namespace thrill_gpu
 
