@@ -16,14 +16,14 @@
  * Device buffers passed in must be 16-byte aligned.  There is NO CPU fallback anywhere behind this ABI.
  *
  * Limits (TG_ERR_TOO_LARGE, checked before any work): every entry point that takes a device item count (tg_radix_sort_local,
- * tg_classify_scatter, tg_sort_select (per shard), tg_hash_aggregate, tg_hash_partition, tg_range_partition, tg_sort, tg_reduce_by_key,
+ * tg_classify_scatter, tg_sort_select and tg_exchange_select (per shard), tg_hash_aggregate, tg_hash_partition, tg_sort, tg_reduce_by_key,
  * tg_reduce_to_index and their _file / _dev forms) takes at most 2^30 - 1 items per call and worker (n_local), and a worker receives at most 2^30 - 1
- * items in an exchange: the partition passes count in 30-bit fields.  ReduceToIndex gives each worker fewer than 2^31
+ * items in an exchange (tg_exchange_select included): the partition passes count in 30-bit fields.  ReduceToIndex gives each worker fewer than 2^31
  * indices of the result.  Merge (tg_merge and its forms) takes at most 2^30 - 1 items in a worker's k inputs together, and gives
  * each worker at most 2^30 - 1 items of the result; it merges 2..16 inputs of 8- or 16-byte items.  InnerJoin (tg_inner_join
  * and its _file form) takes at most 2^30 - 1 items per worker and side, before and after its exchange, and gives each worker at
  * most 2^30 - 1 items of the result.  GroupByKey and GroupToIndex (tg_group_by_key, tg_group_to_index and their _file forms)
- * take at most 2^30 - 1 items per worker, before and after their exchange, and tg_mod_partition at most 2^30 - 1 items per call.
+ * take at most 2^30 - 1 items per worker, before and after their exchange.
  * PrefixSum, ExPrefixSum and ZipWithIndex (tg_prefix_sum, tg_zip_with_index, their _file and _select forms, tg_scan_local_total)
  * take at most 2^30 - 1 items per worker and give each worker as many items as it holds.  Sum, Min, Max and AllReduce (tg_all_reduce
  * and its _file and _select forms) take at most 2^30 - 1 items per worker.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
@@ -223,13 +223,6 @@ int tg_hash_aggregate(tg_ctx* ctx, const tg_kv_desc* desc, const void* d_in, siz
 int tg_hash_partition(tg_ctx* ctx, const tg_kv_desc* desc, const void* d_in, size_t n, uint32_t p,
                       void* d_out, uint64_t* out_counts);
 
-/* Range partition of ReduceToIndex (what its exchange classifies by): destination of a 16-byte item with u64 index k is
- * k < size ? k * p / size : p - 1 (core/reduce_functional.hpp:112-125; worker d's range starts at ceil(d * size / p)).  Stable:
- * d_out receives the items grouped by destination in input order, out_counts[p] (host) the counts.  1 <= p <= 256; a size with
- * (size - 1) * p >= 2^64 is TG_ERR_ARG. */
-int tg_range_partition(tg_ctx* ctx, const void* d_in, size_t n, uint64_t size, uint32_t p,
-                       void* d_out, uint64_t* out_counts);
-
 /* The arithmetic of one exchange, pure host code (what every rank derives from the all-gathered p x p count matrix; exported so
  * that the N > 1 host logic is testable without GPUs): counts[src * p + dst] = items rank src holds for rank dst.  For rank `me`:
  * send_cnt[d], recv_cnt[s], recv_before[d] = items of the ranks below `me` in rank d's window (where this rank's share starts),
@@ -237,6 +230,30 @@ int tg_range_partition(tg_ctx* ctx, const void* d_in, size_t n, uint64_t size, u
  * decided on it, identically everywhere).  Replaces the per-(src,dst) block headers of the MixStream (data/multiplexer_header.hpp:36-72). */
 int tg_exchange_plan(uint32_t p, uint32_t me, const uint32_t* counts, uint64_t* send_cnt, uint64_t* recv_cnt,
                      uint64_t* recv_before, uint64_t* n_recv, uint64_t* worst);
+
+/* The exchange of the collective operators for p simulated workers on one device (2 <= p <= 16, any ctx): shard w (n_shards[w]
+ * items at d_shards[w]) is worker w's input, d_windows[d] (window_bytes[d] bytes) worker d's exchange window.  It runs the
+ * operators' device code of the exchange except the all-gather of the counts and the transport: each worker's count step (chunk
+ * histograms of the destination), the count matrix, then each worker's store step, the workers one after another on the ctx's
+ * stream.  Window d receives the items every worker sends to d, grouped by source worker in rank order, each group in the
+ * sender's input order (the layout CatStream delivers).  The route is the destination of an item:
+ *   TG_ROUTE_HASH       Hash128to64(0, key) % p of a 16-byte (u64 key, value) item: ReduceByKey and InnerJoin
+ *   TG_ROUTE_MOD        key % p of a 16-byte item: GroupByKey
+ *   TG_ROUTE_RANGE      k < result_size ? k * p / result_size : p - 1 of a 16-byte item with u64 index k: ReduceToIndex and
+ *                       GroupToIndex ((result_size - 1) * p >= 2^64 is TG_ERR_ARG)
+ *   TG_ROUTE_SPLITTERS  the multi-worker Sort's classification with the splitters tg_sort_select selects for desc and rng_seed:
+ *                       8- or 16-byte items with any descriptor tg_sort takes for them, or records (4-byte aligned, classified by
+ *                       their 16-byte key tuples and moved whole)
+ * desc and rng_seed are used by TG_ROUTE_SPLITTERS only, result_size by TG_ROUTE_RANGE only.  mode 1 is the peer-store pass (the
+ * partition pass storing bucket d straight into window d), mode 0 the two-step form of TG_EXCHANGE=nccl (the local stable
+ * partition, then device-to-device copies of the segments that ncclSend / ncclRecv move).  Writes out_counts[src * p + dst]
+ * first; then a worker receiving 2^30 or more items, or a shard of 2^30 or more items, is TG_ERR_TOO_LARGE; d_windows == NULL
+ * returns the counts only; a window smaller than its receive size is TG_ERR_ARG.  These checks come before any store, and only
+ * [0, receive size) of a window is written.  Shards are read, never modified. */
+enum { TG_ROUTE_HASH = 0, TG_ROUTE_MOD = 1, TG_ROUTE_RANGE = 2, TG_ROUTE_SPLITTERS = 3 };
+int tg_exchange_select(tg_ctx* ctx, uint32_t route, uint32_t mode, const tg_key_desc* desc, uint64_t rng_seed, uint64_t result_size,
+                       const void* const* d_shards, const size_t* n_shards, uint32_t p, void* const* d_windows,
+                       const size_t* window_bytes, uint64_t* out_counts);
 
 /* ---- operator-level entry points -------------------------------------------------------------------- */
 
@@ -397,9 +414,6 @@ int tg_group_to_index(tg_ctx* ctx, const void* d_in, size_t n_local, uint64_t re
 int tg_group_by_key_file(tg_ctx* ctx, const tg_merge_input* in, size_t* out_items);
 int tg_group_to_index_file(tg_ctx* ctx, const tg_merge_input* in, uint64_t result_size, size_t* out_items,
                            uint64_t* out_begin, uint64_t* out_end);
-/* kernel level (tests of the placement on one GPU): GroupByKey's partition, destination of a 16-byte item = key % p.  Stable:
- * d_out receives the items grouped by destination in input order, out_counts[p] (host) the counts.  1 <= p <= 256. */
-int tg_mod_partition(tg_ctx* ctx, const void* d_in, size_t n, uint32_t p, void* d_out, uint64_t* out_counts);
 
 /* ---- PrefixSum / ExPrefixSum / ZipWithIndex: scans by global position (DIA::PrefixSum, DIA::ExPrefixSum, api/dia.hpp:1850,
  * :1867, PrefixSumNode api/prefix_sum.hpp:28-128; DIA::ZipWithIndex, ZipWithIndexNode api/zip_with_index.hpp:40-110) -----------

@@ -1,7 +1,7 @@
-"""GroupByKey / GroupToIndex on one H100: tg_group_by_key, tg_group_to_index, their _file forms, tg_mod_partition and the Python
-mirror against the numpy restatement in group_ref.py (bit-exact: sorted by key, stable within a key) and against the reference's
-outputs in tests/golden/reference_outputs_group.npz, including p = 2, 3, 4 and 8 workers simulated on one GPU through the
-kernel-level partitions; device Files, argument errors and the size limit, a full-size case, the multi-GPU worker and the
+"""GroupByKey / GroupToIndex on one H100: tg_group_by_key, tg_group_to_index, their _file forms and the Python mirror against
+the numpy restatement in group_ref.py (bit-exact: sorted by key, stable within a key) and against the reference's outputs in
+tests/golden/reference_outputs_group.npz (p = 2, 3, 4 and 8 workers simulated on one GPU through the real exchange are in
+test_gpu_exchange.py); device Files, argument errors and the size limit, a full-size case, the multi-GPU worker and the
 in-Thrill test binary where the machine has what they need.  pytest -m gpu."""
 import ctypes as C
 import hashlib
@@ -150,53 +150,6 @@ def test_fixture_shapes_one_worker(ctx):
         assert _same(rows, g["%s/%s_p1" % (name, case)]), (name, case)
 
 
-def _partition(ctx, arr, p, size=None):
-    """tg_mod_partition (size None) or tg_range_partition: the p buckets, each in input order"""
-    d_in, d_out = ctx.to_device(arr), ctx.alloc(max(16, len(arr) * 16))
-    counts = (C.c_uint64 * p)()
-    if size is None:
-        ctx.ck(ctx.L.tg_mod_partition(ctx.h, d_in, len(arr), p, d_out, counts))
-    else:
-        ctx.ck(ctx.L.tg_range_partition(ctx.h, d_in, len(arr), size, p, d_out, counts))
-    out = _download(ctx, d_out, len(arr))
-    ctx.free(d_in)
-    ctx.free(d_out)
-    b = np.concatenate([[0], np.cumsum(list(counts))]).astype(np.int64)
-    return [out[b[d]:b[d + 1]] for d in range(p)]
-
-
-@pytest.mark.parametrize("p", list(range(2, 17)))
-def test_mod_partition(ctx, p):
-    arr = G.make_input(100000, 1 << 62, p)
-    arr["key"][::7] = np.uint64(p * 1000 + 3)           # a popular key
-    arr["key"][::11] |= np.uint64(1 << 63)
-    arr["val"] = np.arange(len(arr))
-    buckets = _partition(ctx, arr, p)
-    own = G.owner_mod(arr["key"], p)
-    for d in range(p):
-        assert np.array_equal(buckets[d].view(np.uint64), arr[own == d].view(np.uint64)), d    # counts and stable order
-
-
-@pytest.mark.parametrize("p", [2, 3, 4, 8])
-def test_simulated_workers_equal_the_reference(ctx, p):
-    """each shard partitioned by the kernel-level partition, bucket d of the shards concatenated in shard order (what the
-    exchange delivers to worker d), grouped at p = 1: worker d's rows are the reference's worker d"""
-    g = _golden()
-    for name, case in _cases(g, p):
-        inp = g[name + "/in"].view(G.KV)
-        size = None if case.startswith("key_") else int(case[6:])
-        parts = [_partition(ctx, s, p, size) for s in G.split_shards(inp, p)]
-        rows = []
-        for d in range(p):
-            recv = np.concatenate([parts[s][d] for s in range(p)])
-            st, res, _, _ = group_dev(ctx, recv)
-            assert st == 0
-            rows.append(_rows(res, case, p, d))
-        key = "%s/%s_p%d" % (name, case, p)
-        assert [len(r) for r in rows] == g[key + "_counts"].tolist(), key
-        assert _same(np.concatenate(rows), g[key]), key
-
-
 # ---- the _file form, device Files, the Python mirror --------------------------------------------------------------------
 def _run_file(ctx, inp, size):
     n, b, e = C.c_size_t(), C.c_uint64(), C.c_uint64()
@@ -289,6 +242,14 @@ def test_python_group_operators():
 
 
 # ---- errors and the size limit -----------------------------------------------------------------------------------------
+def _mod_exchange(ctx, d, n, p):
+    """tg_exchange_select by key % p, counts only: shard 0 holds n items at d, the other shards are empty"""
+    q = max(p, 1)
+    counts = (C.c_uint64 * (q * q))()
+    return ctx.L.tg_exchange_select(ctx.h, _capi().ROUTE_MOD, 1, None, 0, 0, (C.c_void_p * q)(d, *([None] * (q - 1))),
+                                    (C.c_size_t * q)(n, *([0] * (q - 1))), p, None, None, counts)
+
+
 def test_argument_errors(ctx):
     capi = _capi()
     out, n, b, e = C.c_void_p(), C.c_size_t(), C.c_uint64(), C.c_uint64()
@@ -304,9 +265,9 @@ def test_argument_errors(ctx):
     ob, onb, _ = make_blocks(capi, raw40, 40)
     oin = capi.MergeInput(None, C.cast(ob, C.POINTER(capi.Block)), onb)
     assert ctx.L.tg_group_to_index_file(ctx.h, C.byref(oin), 10, C.byref(n), C.byref(b), C.byref(e)) == TG_ERR_ARG
-    counts = (C.c_uint64 * 300)()
-    assert ctx.L.tg_mod_partition(ctx.h, d, 3, 0, d, counts) == TG_ERR_ARG
-    assert ctx.L.tg_mod_partition(ctx.h, d, 3, 257, d, counts) == TG_ERR_ARG
+    # GroupByKey's exchange (the key % p route) takes 2..16 workers
+    for p in (0, 1, 17):
+        assert _mod_exchange(ctx, d, 3, p) == TG_ERR_ARG, p
     ctx.free(d)
     check(ctx, arr)                                          # the ctx still works
 
@@ -326,8 +287,8 @@ def test_input_over_the_limit_is_too_large(ctx):
     # 2^30 items are refused before anything is allocated or read (the buffer holds one)
     assert ctx.L.tg_group_by_key(ctx.h, d, 1 << 30, C.byref(out), C.byref(n)) == TG_ERR_TOO_LARGE
     assert ctx.L.tg_group_to_index(ctx.h, d, 1 << 30, 10, C.byref(out), C.byref(n), C.byref(b), C.byref(e)) == TG_ERR_TOO_LARGE
-    counts = (C.c_uint64 * 4)()
-    assert ctx.L.tg_mod_partition(ctx.h, d, 1 << 30, 4, d, counts) == TG_ERR_TOO_LARGE
+    # ... and by the exchange (a worker's shard of 2^30 items: its count step reads nothing)
+    assert _mod_exchange(ctx, d, 1 << 30, 4) == TG_ERR_TOO_LARGE
     ctx.free(d)
 
 

@@ -1,7 +1,7 @@
-"""The multi-worker Sort's device classification and ReduceToIndex's range partition on one H100, bit-exact against
-sample_sort_ref: tg_sort_select runs the operator's sampling, splitter selection, top-byte lookup table, SplitterDigit pass
-(with the global index base the selection writes on the device) and the merge pipeline's boundaries for p simulated workers;
-tg_range_partition runs RangeDigit.  pytest -m gpu."""
+"""The multi-worker Sort's device classification on one H100, bit-exact against sample_sort_ref: tg_sort_select runs the
+operator's sampling, splitter selection, top-byte lookup table, SplitterDigit pass (with the global index base the selection
+writes on the device) and the merge pipeline's boundaries for p simulated workers.  (ReduceToIndex's range route and the
+exchange's stores are tested through tg_exchange_select in test_gpu_exchange.py.)  pytest -m gpu."""
 import ctypes as C
 
 import numpy as np
@@ -119,37 +119,6 @@ def test_worker_counts_and_shard_shapes(ctx, d, p):
             raise AssertionError("%s: %s" % (name, e))
 
 
-# ---- range partition --------------------------------------------------------------------------------------------------------
-def range_keys(rng, n, size, p):
-    keys = rng.randint(0, size, size=n, dtype=np.int64).astype(np.uint64)
-    edges = sorted({S.begin_of_part(r, size, p) + o for r in range(p + 1) for o in (-1, 0, 1)} | {size, (1 << 64) - 1})
-    special = np.array([e for e in edges if 0 <= e < (1 << 64)], dtype=np.uint64)
-    at = rng.randint(0, n, size=min(n, 3 * len(special)))
-    keys[at] = special[np.arange(len(at)) % len(special)]
-    return keys
-
-
-@pytest.mark.parametrize("p", [2, 3, 7, 16])
-def test_range_partition(ctx, p):
-    rng = np.random.RandomState(p)
-    for size in (1, p - 1, p, p + 1, 1000, (1 << 34) + 3):
-        for n in (8191, 8192, 8193, 3 * 8192 + 1):
-            items = np.zeros(n, dtype=[("k", "<u8"), ("v", "<u8")])
-            items["k"] = range_keys(rng, n, size, p)
-            items["v"] = np.arange(n, dtype=np.uint64)                  # the input position shows the order within a destination
-            rows = R.rows(items, 16)
-            din, dout = ctx.to_device(rows), ctx.alloc(n * 16)
-            counts = np.zeros(p, np.uint64)
-            st = ctx.L.tg_range_partition(ctx.h, din, n, size, p, dout, _u64p(counts))
-            assert st == 0, ctx.L.tg_last_error(ctx.h)
-            got = ctx.download(dout, n * 16).reshape(-1, 16)
-            ctx.free(din)
-            ctx.free(dout)
-            want, want_counts = S.range_partition(rows, size, p)
-            assert np.array_equal(counts, want_counts), (size, n)
-            assert np.array_equal(got, want), (size, n)
-
-
 # ---- arguments ----------------------------------------------------------------------------------------------------------------
 def test_argument_errors(ctx):
     L = ctx.L
@@ -180,13 +149,22 @@ def test_argument_errors(ctx):
     assert L.tg_sort_select(ctx.h, C.byref(d), P, (C.c_size_t * 2)(100, 5), 2, 1, spl.ctypes.data,
                             (C.c_void_p * 2)(out, out), _u64p(counts), None) == TG_ERR_ARG           # a NULL shard of 5 items
     assert call(3, n=1 << 30) == TG_ERR_TOO_LARGE
-    rc = np.zeros(300, np.uint64)
-    for p in (0, 257):
-        assert L.tg_range_partition(ctx.h, dev, 50, 1000, p, out, _u64p(rc)) == TG_ERR_ARG
-    assert L.tg_range_partition(ctx.h, dev, 50, 1000, 4, out, None) == TG_ERR_ARG
-    assert L.tg_range_partition(ctx.h, None, 50, 1000, 4, out, _u64p(rc)) == TG_ERR_ARG
-    assert L.tg_range_partition(ctx.h, dev, 50, (1 << 62) + 2, 4, out, _u64p(rc)) == TG_ERR_ARG      # k * p would overflow
-    assert L.tg_range_partition(ctx.h, dev, 1 << 30, 1000, 4, out, _u64p(rc)) == TG_ERR_TOO_LARGE
+    # ReduceToIndex's range route through the exchange (counts only): 2..16 workers, the counts, a shard pointer where there are
+    # items, (size - 1) * p < 2^64, shards below 2^30 items
+    rc = np.zeros(17 * 17, np.uint64)
+
+    def rng_call(p, shard=dev, n=50, size=1000, cnt=True):
+        q = max(p, 1)
+        return L.tg_exchange_select(ctx.h, _capi().ROUTE_RANGE, 1, None, 0, size, (C.c_void_p * q)(shard, *([None] * (q - 1))),
+                                    (C.c_size_t * q)(n, *([0] * (q - 1))), p, None, None, _u64p(rc) if cnt else None)
+
+    for p in (0, 1, 17):
+        assert rng_call(p) == TG_ERR_ARG, p
+    assert rng_call(4, cnt=False) == TG_ERR_ARG
+    assert rng_call(4, shard=None) == TG_ERR_ARG
+    assert rng_call(4, size=(1 << 62) + 2) == TG_ERR_ARG                # k * p would overflow
+    assert rng_call(4, n=1 << 30) == TG_ERR_TOO_LARGE
+    assert rng_call(4) == 0 and rc[:16].tolist() == [50] + [0] * 15     # 50 items, indices 0, 2, .., 98 of 1000: worker 0
     ctx.free(dev)
     ctx.free(out)
     # the ctx still works

@@ -15,6 +15,7 @@ OP_SUM_F64, OP_SUM_U64, OP_MIN_U64, OP_MAX_U64, OP_MIN_F64, OP_MAX_F64, OP_FIRST
 K_RADIX_HIST, K_PARTITION, K_MERGE, K_PREAGG, K_AGGREGATE, K_COMPACT, K_OTHER, K_FIXUP, K_SEGCOUNT, K_EXCHANGE, K_JOIN, K_SCAN = \
     range(12)
 JOIN_KEY_VALUES, JOIN_VALUES = 0, 1
+ROUTE_HASH, ROUTE_MOD, ROUTE_RANGE, ROUTE_SPLITTERS = range(4)
 
 
 class KeyDesc(C.Structure):
@@ -105,8 +106,8 @@ SYMBOLS = [
     ("tg_kway_merge", _i, [_vp, _P(KeyDesc), _vp, _P(_u64), _u32, _vp, _vp]),
     ("tg_hash_aggregate", _i, [_vp, _P(KVDesc), _vp, _sz, _vp, _P(_u64)]),
     ("tg_hash_partition", _i, [_vp, _P(KVDesc), _vp, _sz, _u32, _vp, _P(_u64)]),
-    ("tg_range_partition", _i, [_vp, _vp, _sz, _u64, _u32, _vp, _P(_u64)]),
     ("tg_exchange_plan", _i, [_u32, _u32, _P(_u32), _P(_u64), _P(_u64), _P(_u64), _P(_u64), _P(_u64)]),
+    ("tg_exchange_select", _i, [_vp, _u32, _u32, _P(KeyDesc), _u64, _u64, _P(_vp), _P(_sz), _u32, _P(_vp), _P(_sz), _P(_u64)]),
     ("tg_sort", _i, [_vp, _P(KeyDesc), _vp, _sz, _u64, _P(_vp), _P(_sz)]),
     ("tg_reduce_by_key", _i, [_vp, _P(KVDesc), _vp, _sz, _P(_vp), _P(_sz)]),
     ("tg_reduce_to_index", _i, [_vp, _P(KVDesc), _vp, _sz, _u64, _vp, _P(_vp), _P(_sz), _P(_u64)]),
@@ -130,7 +131,6 @@ SYMBOLS = [
     ("tg_group_to_index", _i, [_vp, _vp, _sz, _u64, _P(_vp), _P(_sz), _P(_u64), _P(_u64)]),
     ("tg_group_by_key_file", _i, [_vp, _P(MergeInput), _P(_sz)]),
     ("tg_group_to_index_file", _i, [_vp, _P(MergeInput), _u64, _P(_sz), _P(_u64), _P(_u64)]),
-    ("tg_mod_partition", _i, [_vp, _vp, _sz, _u32, _vp, _P(_u64)]),
     ("tg_prefix_sum", _i, [_vp, _P(ScanDesc), _vp, _sz, _vp, _i, _P(_vp), _P(_sz)]),
     ("tg_zip_with_index", _i, [_vp, _vp, _sz, _i, _P(_vp), _P(_sz)]),
     ("tg_prefix_sum_file", _i, [_vp, _P(ScanDesc), _P(MergeInput), _vp, _i, _P(_sz)]),

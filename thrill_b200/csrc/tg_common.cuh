@@ -53,7 +53,6 @@ struct tg_ctx {
         size_t cap = 0;                        // bytes; the same on every rank (grown collectively)
         void* peer[TG_MAX_RANKS] = { nullptr };
         bool ipc_open[TG_MAX_RANKS] = { false };
-        void** d_peer = nullptr;               // device scratch: [0..p) destination base pointers of the current exchange
         int mode = -1;                         // -1 not negotiated yet, 0 = NCCL send/recv, 1 = P2P stores
     } xwin;
     uint64_t hot_records = 0;                    // records folded by the counting reads of the aggregations (tg_hot_records)

@@ -133,7 +133,6 @@ int xwin_negotiate(tg_ctx* ctx) {
     if (w.mode >= 0) return TG_OK;
     const char* e = getenv("TG_EXCHANGE");
     if (e && !strcmp(e, "nccl")) w.mode = 0;
-    if (!w.d_peer) TG_CUDA(ctx, cudaMalloc((void**)&w.d_peer, PEER_MAX * sizeof(void*)));
     return remap(ctx, (size_t)1 << 20);
 }
 
@@ -169,30 +168,51 @@ int xchg_counts(tg_ctx* ctx, const u32* d_totals, int item_bytes, XchgResult* re
     return TG_OK;
 }
 
+const u32* xchg_matrix(tg_ctx* ctx) { return (const u32*)ctx->pinned + 16384; }
+
 // destination pointers of the peer-store pass.  Bucket d of the local partition would start at gbase[d] = sum of the
 // send counts below d; in worker d's window this worker's items start after those of the lower ranks.  dbase[d] is biased
-// by -gbase[d] so that the pass can use the positions it computes for a local output.
-int xchg_upload_dest(tg_ctx* ctx, int item_bytes, const XchgResult& res, void*** d_dbase_out) {
-    const int p = ctx->nranks, me = ctx->rank;
-    const u32* h_mat = (const u32*)ctx->pinned + 16384;
-    u64* h_ptr = (u64*)ctx->pinned + 9216;      // byte offset 72 KB
+// by -gbase[d] so that the pass can use the positions it computes for a local output.  Staged through the pinned scratch
+// (byte offset 72 KB) into the control workspace (byte offset 80 KB): the next upload must wait for this one's copy.
+int xchg_upload_dest(tg_ctx* ctx, const u32* counts, int p, int me, int item_bytes, void* const* windows, void*** d_dbase_out) {
+    u64* h_ptr = (u64*)ctx->pinned + 9216;
+    char* d;
+    TG_TRY(tg_ws_get(ctx, WS_XCTL, 1 << 17, (void**)&d));
+    void** d_dbase = (void**)(d + (80 << 10));
     u64 gbase = 0, before[TG_MAX_RANKS], sc[TG_MAX_RANKS], rc[TG_MAX_RANKS], nr, worst;
-    tg_exchange_plan((u32)p, (u32)me, h_mat, (uint64_t*)sc, (uint64_t*)rc, (uint64_t*)before, (uint64_t*)&nr, (uint64_t*)&worst);
+    tg_exchange_plan((u32)p, (u32)me, counts, (uint64_t*)sc, (uint64_t*)rc, (uint64_t*)before, (uint64_t*)&nr, (uint64_t*)&worst);
     for (int d = 0; d < PEER_MAX; ++d) {
         if (d >= p) { h_ptr[d] = 0; continue; }
-        h_ptr[d] = (u64)(uintptr_t)ctx->xwin.peer[d] + (before[d] - gbase) * (u64)item_bytes;   // (64-bit: wraps like the pass's positions)
-        gbase += res.send_cnt[d];
+        h_ptr[d] = (u64)(uintptr_t)windows[d] + (before[d] - gbase) * (u64)item_bytes;   // (64-bit: wraps like the pass's positions)
+        gbase += sc[d];
     }
-    TG_CUDA(ctx, cudaMemcpyAsync(ctx->xwin.d_peer, h_ptr, PEER_MAX * sizeof(void*), cudaMemcpyHostToDevice, ctx->stream));
-    *d_dbase_out = ctx->xwin.d_peer;
+    TG_CUDA(ctx, cudaMemcpyAsync(d_dbase, h_ptr, PEER_MAX * sizeof(void*), cudaMemcpyHostToDevice, ctx->stream));
+    *d_dbase_out = d_dbase;
     return TG_OK;
 }
 
-// after xchg_counts: this worker's items start at item before[d] of worker d's window
-void xchg_recv_offsets(tg_ctx* ctx, u64* before) {
-    const u32* h_mat = (const u32*)ctx->pinned + 16384;
-    u64 sc[TG_MAX_RANKS], rc[TG_MAX_RANKS], nr, worst;
-    tg_exchange_plan((u32)ctx->nranks, (u32)ctx->rank, h_mat, (uint64_t*)sc, (uint64_t*)rc, (uint64_t*)before, (uint64_t*)&nr, (uint64_t*)&worst);
+int xchg_transfer(tg_ctx* ctx, bool simulated, const void* d_part, size_t s, const u32* counts, int p, int me, void* const* windows) {
+    u64 before[TG_MAX_RANKS], sc[TG_MAX_RANKS], rc[TG_MAX_RANKS], nr, worst;
+    tg_exchange_plan((u32)p, (u32)me, counts, (uint64_t*)sc, (uint64_t*)rc, (uint64_t*)before, (uint64_t*)&nr, (uint64_t*)&worst);
+    u64 soff = 0, roff = 0;
+    if (simulated) {
+        // what ncclSend(segment d) / ncclRecv on worker d put there: the same bytes at the same place of worker d's window
+        for (int d = 0; d < p; ++d) {
+            if (sc[d]) TG_CUDA(ctx, cudaMemcpyAsync((char*)windows[d] + before[d] * s, (const char*)d_part + soff * s, sc[d] * s,
+                                                    cudaMemcpyDeviceToDevice, ctx->stream));
+            soff += sc[d];
+        }
+        return TG_OK;
+    }
+    TG_NCCL(ctx, ncclGroupStart());
+    for (int r = 0; r < p; ++r) {
+        if (sc[r]) TG_NCCL(ctx, ncclSend((const char*)d_part + soff * s, sc[r] * s, ncclUint8, r, ctx->comm, ctx->stream));
+        if (rc[r]) TG_NCCL(ctx, ncclRecv((char*)ctx->xwin.base + roff * s, rc[r] * s, ncclUint8, r, ctx->comm, ctx->stream));
+        soff += sc[r];
+        roff += rc[r];
+    }
+    TG_NCCL(ctx, ncclGroupEnd());
+    return TG_OK;
 }
 
 int evacuate_window_inputs(tg_ctx* ctx, const void** in, const size_t* bytes, uint32_t k) {
@@ -230,7 +250,6 @@ int sort_pairs_into(tg_ctx* ctx, int slot, const void* src, u64 n, const ulonglo
 void xwin_release(tg_ctx* ctx) {
     unmap_peers(ctx);
     if (ctx->xwin.base) cudaFree(ctx->xwin.base);
-    if (ctx->xwin.d_peer) cudaFree(ctx->xwin.d_peer);
     ctx->xwin = tg_ctx::XWin();
 }
 

@@ -32,8 +32,13 @@ int xwin_negotiate(tg_ctx* ctx);                                    // collectiv
 int xwin_ensure(tg_ctx* ctx, size_t bytes_all_ranks);               // collective: every rank's window >= bytes
 int xwin_barrier(tg_ctx* ctx);                                      // stream-ordered cross-rank barrier
 int xchg_counts(tg_ctx* ctx, const u32* d_totals, int item_bytes, XchgResult* res, u64* need_bytes_max);
-int xchg_upload_dest(tg_ctx* ctx, int item_bytes, const XchgResult& res, void*** d_dbase_out);
-void xchg_recv_offsets(tg_ctx* ctx, u64* before);                  // before[d] = items of the lower ranks in worker d's window
+const u32* xchg_matrix(tg_ctx* ctx);                                // after xchg_counts: the p x p count matrix (host)
+// the destination pointers of worker me's peer-store pass (device, PEER_MAX pointers in a workspace slot)
+int xchg_upload_dest(tg_ctx* ctx, const u32* counts, int p, int me, int item_bytes, void* const* windows, void*** d_dbase_out);
+// the transfers of the two-step form: segment d of worker me's destination-grouped items d_part goes to worker d's window,
+// after the items of the lower ranks (ncclSend / ncclRecv into this rank's window, or simulated: device copies into windows[d])
+int xchg_transfer(tg_ctx* ctx, bool simulated, const void* d_part, size_t item_bytes, const u32* counts, int p, int me,
+                  void* const* windows);
 // inputs that lie inside the exchange window (an un-detached result of the previous collective operator) are moved out of
 // the peers' way first (into WS_AUX): the span they cover is copied once, so that inputs sharing it stay consistent
 int evacuate_window_inputs(tg_ctx* ctx, const void** in, const size_t* bytes, uint32_t k);
@@ -86,18 +91,23 @@ struct RangeDigit {
 // answers for [range_begin(r), range_begin(r + 1)), the indices RangeDigit sends to it
 inline u64 range_begin(u64 r, u64 size, u64 p) { return (u64)(((unsigned __int128)r * size + p - 1) / p); }
 
-// Stable partition of n local items by fn (destination worker, < p) + Alltoallv.  Collective.
-// n >= 2^30 (over the per-call limit): this rank sends nothing and reports 2^30 items for worker 0 in its counts, so that
-// xchg_counts returns TG_ERR_TOO_LARGE on every rank and none is left waiting in a collective.
+// What the count step of one exchange leaves for its store step: the chunk geometry of the worker's pass and, in WS_SORT_HIST2,
+// its per-destination totals and per-chunk bases.
+struct XchgLocal {
+    size_t n = 0;                   // items that take part (0 for a worker over the limit)
+    ChunkGeom g = { 0, 0 };
+    u32* totals = nullptr;          // [RADIX] (device): items for each destination worker
+    u32* chunkbase = nullptr;       // [nchunks][RADIX] (device): where each chunk's bucket d starts in the grouped order
+};
+
+// Count step of one exchange: destination histograms per chunk (chunk_hist_kernel) and their scan (chunk_scan_kernel).
+// n >= 2^30 (over the per-call limit): the worker takes part with no items and reports 2^30 items for worker 0 in its totals,
+// so that the plan of the count matrix gives TG_ERR_TOO_LARGE on every rank and none is left waiting in a collective.
 template <int WORDS, class DigitFn>
-int exchange_scatter(tg_ctx* ctx, const void* d_in, size_t n, const DigitFn& fn, XchgResult* res) {
+int exchange_count(tg_ctx* ctx, const void* d_in, size_t n, const DigitFn& fn, XchgLocal* xl) {
     typedef typename ItemT<WORDS>::type Item;
-    const int p = ctx->nranks;
-    const size_t s = sizeof(Item);
     const bool too_large = n >= (1u << 30);
     if (too_large) n = 0;
-    TG_TRY(xwin_negotiate(ctx));
-    // (1) destination histogram per chunk
     const ChunkGeom g = chunk_geometry<WORDS>(ctx, n);
     const size_t cw = (size_t)(g.nchunks > 0 ? g.nchunks : 1) * RADIX;
     u32* tab;
@@ -112,36 +122,28 @@ int exchange_scatter(tg_ctx* ctx, const void* d_in, size_t n, const DigitFn& fn,
     }
     else TG_CUDA(ctx, cudaMemsetAsync(totals, 0, 2 * RADIX * 4, ctx->stream));
     if (too_large) TG_CUDA(ctx, cudaMemsetAsync((char*)totals + 3, 0x40, 1, ctx->stream));     // totals[0] = 0x40000000 = 2^30
-    // (2) count matrix; every rank learns every rank's receive size
-    u64 need = 0;
-    TG_TRY(xchg_counts(ctx, totals, (int)s, res, &need));
-    TG_TRY(xwin_ensure(ctx, need));
-    res->d_recv = ctx->xwin.base;
-    if (ctx->xwin.mode == 1) {
-        // (3) classification + scatter + Alltoallv in one pass: stores into the peers' windows
-        if (n) {
-            void** d_dbase;
-            TG_TRY(xchg_upload_dest(ctx, (int)s, *res, &d_dbase));
-            std::vector<u32> chunk_size(g.nchunks, g.chunk_items);
-            chunk_size[g.nchunks - 1] = (u32)(n - (size_t)(g.nchunks - 1) * g.chunk_items);
-            uint4* d_tiles;
-            u32 total = 0;
-            TG_TRY(build_tile_list(ctx, g.nchunks, chunk_size.data(), tile_items<WORDS>(), 0, WS_SEG_TILES2, &d_tiles, &total));
-            u32* status;
-            TG_TRY(tg_ws_get(ctx, WS_SORT_STATUS, (size_t)total * RADIX * 4, (void**)&status));
-            TG_CUDA(ctx, cudaMemsetAsync(status, 0, (size_t)total * RADIX * 4, ctx->stream));
-            SegList sl = { d_tiles, chunkbase, total, nullptr };
-            const int xprof = ctx->profile ? tg_prof_begin(ctx, TG_K_EXCHANGE) : -1;
-            TG_TRY((launch_partition_peer<WORDS, DigitFn>(ctx, d_in, (u32)n, fn, status, sl, (Item* const*)d_dbase)));
-            if (xprof >= 0) tg_prof_end(ctx, xprof);
-        }
-        // (4) every peer's stores into this window are complete after the barrier
-        TG_TRY(xwin_barrier(ctx));
-        return TG_OK;
-    }
-    // two-step form: local stable partition, then grouped send/recv into the window
-    void* d_part;
-    TG_TRY(tg_ws_get(ctx, WS_XCHG_SEND, (n + 2) * s, &d_part));
+    xl->n = n;
+    xl->g = g;
+    xl->totals = totals;
+    xl->chunkbase = chunkbase;
+    return TG_OK;
+}
+
+// Store step of one exchange for worker `me` of p, after its count step (xl): counts = the p x p count matrix (host,
+// counts[src * p + dst]), windows[d] = worker d's window as this process addresses it.
+//   mode 1  the peer-store pass: bucket d straight into windows[d], after the items of the lower ranks
+//   mode 0  the local stable partition into WS_XCHG_SEND, then the per-(src, dst) transfers (xchg_transfer)
+// The receive sizes must have been checked against the windows (the plan's `worst`) before.
+template <int WORDS, class DigitFn>
+int exchange_store(tg_ctx* ctx, int mode, bool simulated, const void* d_in, const XchgLocal& xl, const DigitFn& fn, const u32* counts,
+                   int p, int me, void* const* windows) {
+    typedef typename ItemT<WORDS>::type Item;
+    const size_t s = sizeof(Item), n = xl.n;
+    const ChunkGeom& g = xl.g;
+    void** d_dbase = nullptr;
+    void* d_part = nullptr;
+    if (mode == 1) { if (n) TG_TRY(xchg_upload_dest(ctx, counts, p, me, (int)s, windows, &d_dbase)); }
+    else TG_TRY(tg_ws_get(ctx, WS_XCHG_SEND, (n + 2) * s, &d_part));
     if (n) {
         std::vector<u32> chunk_size(g.nchunks, g.chunk_items);
         chunk_size[g.nchunks - 1] = (u32)(n - (size_t)(g.nchunks - 1) * g.chunk_items);
@@ -151,20 +153,43 @@ int exchange_scatter(tg_ctx* ctx, const void* d_in, size_t n, const DigitFn& fn,
         u32* status;
         TG_TRY(tg_ws_get(ctx, WS_SORT_STATUS, (size_t)total * RADIX * 4, (void**)&status));
         TG_CUDA(ctx, cudaMemsetAsync(status, 0, (size_t)total * RADIX * 4, ctx->stream));
-        SegList sl = { d_tiles, chunkbase, total, nullptr };
-        TG_TRY((launch_partition_seg<WORDS, DigitFn>(ctx, d_in, d_part, (u32)n, fn, status, sl)));
+        SegList sl = { d_tiles, xl.chunkbase, total, nullptr };
+        if (mode == 1) {
+            // classification + scatter + Alltoallv in one pass: stores into the peers' windows
+            const int xprof = ctx->profile ? tg_prof_begin(ctx, TG_K_EXCHANGE) : -1;
+            TG_TRY((launch_partition_peer<WORDS, DigitFn>(ctx, d_in, (u32)n, fn, status, sl, (Item* const*)d_dbase)));
+            if (xprof >= 0) tg_prof_end(ctx, xprof);
+        }
+        else TG_TRY((launch_partition_seg<WORDS, DigitFn>(ctx, d_in, d_part, (u32)n, fn, status, sl)));
     }
+    if (mode == 1) return TG_OK;
     const int xprof = ctx->profile ? tg_prof_begin(ctx, TG_K_EXCHANGE) : -1;
-    TG_NCCL(ctx, ncclGroupStart());
-    u64 soff = 0, roff = 0;
-    for (int r = 0; r < p; ++r) {
-        if (res->send_cnt[r]) TG_NCCL(ctx, ncclSend((const char*)d_part + soff * s, res->send_cnt[r] * s, ncclUint8, r, ctx->comm, ctx->stream));
-        if (res->recv_cnt[r]) TG_NCCL(ctx, ncclRecv((char*)res->d_recv + roff * s, res->recv_cnt[r] * s, ncclUint8, r, ctx->comm, ctx->stream));
-        soff += res->send_cnt[r];
-        roff += res->recv_cnt[r];
-    }
-    TG_NCCL(ctx, ncclGroupEnd());
+    TG_TRY(xchg_transfer(ctx, simulated, d_part, s, counts, p, me, windows));
     if (xprof >= 0) tg_prof_end(ctx, xprof);
+    return TG_OK;
+}
+
+// Stable partition of n local items by fn (destination worker, < p) + Alltoallv.  Collective.
+// n >= 2^30 (over the per-call limit): this rank sends nothing and reports 2^30 items for worker 0 in its counts, so that
+// xchg_counts returns TG_ERR_TOO_LARGE on every rank and none is left waiting in a collective.
+template <int WORDS, class DigitFn>
+int exchange_scatter(tg_ctx* ctx, const void* d_in, size_t n, const DigitFn& fn, XchgResult* res) {
+    typedef typename ItemT<WORDS>::type Item;
+    const size_t s = sizeof(Item);
+    TG_TRY(xwin_negotiate(ctx));
+    // (1) destination histogram per chunk
+    XchgLocal xl;
+    TG_TRY((exchange_count<WORDS, DigitFn>(ctx, d_in, n, fn, &xl)));
+    // (2) count matrix; every rank learns every rank's receive size
+    u64 need = 0;
+    TG_TRY(xchg_counts(ctx, xl.totals, (int)s, res, &need));
+    TG_TRY(xwin_ensure(ctx, need));
+    res->d_recv = ctx->xwin.base;
+    // (3) the stores into the peers' windows (or the local partition and the send/recv into the window)
+    TG_TRY((exchange_store<WORDS, DigitFn>(ctx, ctx->xwin.mode, false, d_in, xl, fn, xchg_matrix(ctx), ctx->nranks, ctx->rank,
+                                           ctx->xwin.peer)));
+    // (4) every peer's stores into this window are complete after the barrier
+    if (ctx->xwin.mode == 1) TG_TRY(xwin_barrier(ctx));
     return TG_OK;
 }
 

@@ -99,21 +99,6 @@ int stage_input(tg_ctx* ctx, const tg_merge_input* in, const void** d_in, size_t
 
 extern "C" {
 
-int tg_mod_partition(tg_ctx* ctx, const void* d_in, size_t n, uint32_t p, void* d_out, uint64_t* out_counts) {
-    if (!ctx || p == 0 || p > RADIX || !out_counts || (n && (!d_in || !d_out)))
-        return tg_set_error(ctx, TG_ERR_ARG, "mod_partition: p=%u or a NULL argument", p);
-    if (n >= GROUP_LIMIT) return tg_set_error(ctx, TG_ERR_TOO_LARGE, "mod_partition: n=%zu", n);
-    TG_CUDA(ctx, cudaSetDevice(ctx->device));
-    const ModDigit fn = ModDigit::make(p);
-    u32* d_counts = nullptr;
-    TG_TRY((partition_chunked<2, ModDigit>(ctx, d_in, d_out, n, fn, &d_counts, nullptr)));
-    u32* hc = (u32*)ctx->pinned;
-    TG_CUDA(ctx, cudaMemcpyAsync(hc, d_counts, RADIX * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    for (uint32_t r = 0; r < p; ++r) out_counts[r] = hc[r];
-    return TG_OK;
-}
-
 int tg_group_by_key(tg_ctx* ctx, const void* d_in, size_t n_local, void** out_dptr, size_t* out_n) {
     if (!ctx || !out_dptr || !out_n || (!d_in && n_local)) return tg_set_error(ctx, TG_ERR_ARG, "group_by_key: NULL argument");
     TG_TRY(check_ranks(ctx));

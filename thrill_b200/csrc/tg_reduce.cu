@@ -898,22 +898,6 @@ int tg_hash_partition(tg_ctx* ctx, const tg_kv_desc* desc, const void* d_in, siz
     return TG_OK;
 }
 
-int tg_range_partition(tg_ctx* ctx, const void* d_in, size_t n, uint64_t size, uint32_t p, void* d_out, uint64_t* out_counts) {
-    if (!ctx || p == 0 || p > RADIX || !out_counts || (n && (!d_in || !d_out)))
-        return tg_set_error(ctx, TG_ERR_ARG, "range_partition: p=%u or a NULL argument", p);
-    if (size && size - 1 > ~0ull / p) return tg_set_error(ctx, TG_ERR_ARG, "range_partition: k * p overflows for size=%llu", (unsigned long long)size);
-    if (n >= (1u << 30)) return tg_set_error(ctx, TG_ERR_TOO_LARGE, "range_partition: n=%zu", n);
-    TG_CUDA(ctx, cudaSetDevice(ctx->device));
-    RangeDigit fn = { size, p };
-    u32* d_counts = nullptr;
-    TG_TRY((partition_chunked<2, RangeDigit>(ctx, d_in, d_out, n, fn, &d_counts, nullptr)));
-    u32* hc = (u32*)ctx->pinned;
-    TG_CUDA(ctx, cudaMemcpyAsync(hc, d_counts, RADIX * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    for (uint32_t r = 0; r < p; ++r) out_counts[r] = hc[r];
-    return TG_OK;
-}
-
 int tg_reduce_by_key(tg_ctx* ctx, const tg_kv_desc* desc, const void* d_in, size_t n_local, void** out_dptr, size_t* out_n) {
     TG_TRY(check_kv(ctx, desc));
     if (!out_dptr || !out_n) return TG_ERR_ARG;

@@ -656,6 +656,41 @@ int sort_records_local(tg_ctx* ctx, const tg_key_desc* desc, const tg_key_desc& 
     return TG_OK;
 }
 
+// Store step of the records' exchange for worker `me` of p: d_ptup = its n tuples partitioned by destination, counts = the p x p
+// count matrix (host), windows[d] = worker d's window.  Mode 1 stores the records straight into the windows, mode 0 into the
+// local send buffer (WS_XCHG_SEND) followed by the transfers (xchg_transfer).
+int exchange_store_records(tg_ctx* ctx, int mode, bool simulated, const void* d_in, u32 rb, const ulonglong2* d_ptup, size_t n,
+                           const u32* counts, int p, int me, void* const* windows) {
+    u64 before[TG_MAX_RANKS], send_cnt[TG_MAX_RANKS], rc[TG_MAX_RANKS], nr, worst;
+    tg_exchange_plan((u32)p, (u32)me, counts, (uint64_t*)send_cnt, (uint64_t*)rc, (uint64_t*)before, (uint64_t*)&nr, (uint64_t*)&worst);
+    u64 first[TG_MAX_RANKS + 1];                 // first tuple of every destination in the partitioned tuple array
+    first[0] = 0;
+    for (int d = 0; d < TG_MAX_RANKS; ++d) first[d + 1] = first[d] + (d < p ? send_cnt[d] : 0);
+    const int xprof = ctx->profile ? tg_prof_begin(ctx, TG_K_EXCHANGE) : -1;
+    if (mode == 1) {
+        // one launch per destination, every worker starting with its right-hand neighbour: at any time each window is written by
+        // one peer (all workers going through the destinations in the same order would queue up on one NVLink ingress after the other)
+        for (int k = 0; k < p; ++k) {
+            const int d = (me + 1 + k) % p;
+            u32* dst = (u32*)((char*)windows[d] + before[d] * rb);
+            if (send_cnt[d])
+                TG_LAUNCH(ctx, scatter_records_kernel, ctx->sm_count * 8, 256, 0, (const u32*)d_in, d_ptup + first[d],
+                          (u32)send_cnt[d], rb / 4, 0u, dst);
+        }
+    }
+    else {
+        char* d_send;
+        TG_TRY(tg_ws_get(ctx, WS_XCHG_SEND, (n + 1) * (size_t)rb, (void**)&d_send));
+        for (int d = 0; d < p; ++d)
+            if (send_cnt[d])
+                TG_LAUNCH(ctx, scatter_records_kernel, ctx->sm_count * 8, 256, 0, (const u32*)d_in, d_ptup + first[d],
+                          (u32)send_cnt[d], rb / 4, 0u, (u32*)(d_send + (size_t)first[d] * rb));
+        TG_TRY(xchg_transfer(ctx, simulated, d_send, rb, counts, p, me, windows));
+    }
+    if (xprof >= 0) tg_prof_end(ctx, xprof);
+    return TG_OK;
+}
+
 int sort_records_impl(tg_ctx* ctx, const tg_key_desc* desc, void* d_in, size_t n_local, uint64_t rng_seed,
                       void** out_dptr, size_t* out_n) {
     const u32 rb = desc->item_bytes;
@@ -697,44 +732,103 @@ int sort_records_impl(tg_ctx* ctx, const tg_key_desc* desc, void* d_in, size_t n
     if (h_ctl[3]) return tg_set_error(ctx, TG_ERR_TOO_LARGE, "sort: a worker holds 2^30 or more records");
     if (h_ctl[1] == 0) { *out_dptr = nullptr; *out_n = 0; return TG_OK; }
     TG_TRY(xwin_ensure(ctx, need));
-    u64 first[TG_MAX_RANKS + 1];                 // first tuple of every destination in the partitioned tuple array
-    first[0] = 0;
-    for (int d = 0; d < TG_MAX_RANKS; ++d) first[d + 1] = first[d] + (d < p ? xr.send_cnt[d] : 0);
-    const int xprof = ctx->profile ? tg_prof_begin(ctx, TG_K_EXCHANGE) : -1;
-    if (ctx->xwin.mode == 1) {
-        u64 before[TG_MAX_RANKS];
-        xchg_recv_offsets(ctx, before);
-        // one launch per destination, every worker starting with its right-hand neighbour: at any time each window is written by
-        // one peer (all workers going through the destinations in the same order would queue up on one NVLink ingress after the other)
-        for (int k = 0; k < p; ++k) {
-            const int d = (me + 1 + k) % p;
-            u32* dst = (u32*)((char*)ctx->xwin.peer[d] + before[d] * rb);
-            if (xr.send_cnt[d])
-                TG_LAUNCH(ctx, scatter_records_kernel, ctx->sm_count * 8, 256, 0, (const u32*)d_in, (const ulonglong2*)d_ptup + first[d],
-                          (u32)xr.send_cnt[d], rb / 4, 0u, dst);
-        }
-        TG_TRY(xwin_barrier(ctx));
-    }
-    else {
-        char* d_send;
-        TG_TRY(tg_ws_get(ctx, WS_XCHG_SEND, (n + 1) * (size_t)rb, (void**)&d_send));
-        for (int d = 0; d < p; ++d)
-            if (xr.send_cnt[d])
-                TG_LAUNCH(ctx, scatter_records_kernel, ctx->sm_count * 8, 256, 0, (const u32*)d_in, (const ulonglong2*)d_ptup + first[d],
-                          (u32)xr.send_cnt[d], rb / 4, 0u, (u32*)(d_send + (size_t)first[d] * rb));
-        TG_NCCL(ctx, ncclGroupStart());
-        u64 roff = 0;
-        for (int r = 0; r < p; ++r) {
-            if (xr.send_cnt[r]) TG_NCCL(ctx, ncclSend(d_send + (size_t)first[r] * rb, xr.send_cnt[r] * rb, ncclUint8, r, ctx->comm, ctx->stream));
-            if (xr.recv_cnt[r]) TG_NCCL(ctx, ncclRecv((char*)ctx->xwin.base + roff * rb, xr.recv_cnt[r] * rb, ncclUint8, r, ctx->comm, ctx->stream));
-            roff += xr.recv_cnt[r];
-        }
-        TG_NCCL(ctx, ncclGroupEnd());
-    }
-    if (xprof >= 0) tg_prof_end(ctx, xprof);
+    TG_TRY(exchange_store_records(ctx, ctx->xwin.mode, false, d_in, rb, d_ptup, n, xchg_matrix(ctx), p, me, ctx->xwin.peer));
+    if (ctx->xwin.mode == 1) TG_TRY(xwin_barrier(ctx));
     // ReceiveItems + SortAndWriteToFile (:665-742) on the received records (grouped by source worker in worker order)
     TG_TRY(sort_records_local(ctx, desc, tdesc, ctx->xwin.base, xr.n_recv, out_dptr));
     *out_n = (size_t)xr.n_recv;
+    return TG_OK;
+}
+
+// ---- tg_exchange_select: one exchange for p simulated workers, one after another on the ctx's stream ----------------------------
+// (never two workers' passes at once: the look-back of the partition pass sizes its grid assuming every CTA is resident)
+
+// after the count steps: out_counts, the receive limit and the windows' sizes, before any store
+int select_check(tg_ctx* ctx, const u32* h_mat, int p, size_t s, void* const* d_windows, const size_t* window_bytes, uint64_t* out_counts) {
+    for (int i = 0; i < p * p; ++i) out_counts[i] = h_mat[i];
+    u64 sc[TG_MAX_RANKS], rc[TG_MAX_RANKS], before[TG_MAX_RANKS], nr, worst;
+    tg_exchange_plan((u32)p, 0, h_mat, (uint64_t*)sc, (uint64_t*)rc, (uint64_t*)before, (uint64_t*)&nr, (uint64_t*)&worst);
+    if (worst >= (1u << 30))
+        return tg_set_error(ctx, TG_ERR_TOO_LARGE, "exchange_select: a worker would receive %llu items (limit 2^30 - 1)", (unsigned long long)worst);
+    if (!d_windows) return TG_OK;
+    if (!window_bytes) return tg_set_error(ctx, TG_ERR_ARG, "exchange_select: windows without their sizes");
+    for (int d = 0; d < p; ++d) {
+        u64 recv = 0;
+        for (int src = 0; src < p; ++src) recv += h_mat[src * p + d];
+        if ((recv && !d_windows[d]) || window_bytes[d] < recv * s)
+            return tg_set_error(ctx, TG_ERR_ARG, "exchange_select: window %d holds %zu bytes, receives %llu", d, window_bytes[d],
+                                (unsigned long long)(recv * s));
+    }
+    return TG_OK;
+}
+
+// 8- or 16-byte items by fn; prep(w) sets up worker w's state of fn (the splitters) before each of its steps
+template <int WORDS, class DigitFn, class Prep>
+int select_items(tg_ctx* ctx, int mode, const void* const* d_shards, const size_t* n_shards, int p, const DigitFn& fn, Prep prep,
+                 void* const* d_windows, const size_t* window_bytes, uint64_t* out_counts) {
+    u32* h_mat = (u32*)ctx->pinned + 16384;          // (the pinned scratch's count matrix, as in xchg_counts)
+    XchgLocal xl;
+    for (int w = 0; w < p; ++w) {
+        TG_TRY(prep(w));
+        TG_TRY((exchange_count<WORDS, DigitFn>(ctx, d_shards[w], n_shards[w], fn, &xl)));
+        TG_CUDA(ctx, cudaMemcpyAsync(h_mat + w * p, xl.totals, (size_t)p * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    TG_TRY(select_check(ctx, h_mat, p, 8 * WORDS, d_windows, window_bytes, out_counts));
+    if (!d_windows) return TG_OK;
+    for (int w = 0; w < p; ++w) {
+        // (the count step again: its chunk bases were overwritten by the next worker's)
+        TG_TRY(prep(w));
+        TG_TRY((exchange_count<WORDS, DigitFn>(ctx, d_shards[w], n_shards[w], fn, &xl)));
+        TG_TRY((exchange_store<WORDS, DigitFn>(ctx, mode, true, d_shards[w], xl, fn, h_mat, p, w, d_windows)));
+        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));        // (the pinned staging of the destination pointers is reused)
+    }
+    return TG_OK;
+}
+
+// records: worker w's tuples, sample and splitters as in sort_records_impl, then the records' store step
+int select_records(tg_ctx* ctx, int mode, const tg_key_desc* desc, uint64_t rng_seed, const void* const* d_shards, const size_t* n_shards,
+                   int p, void* const* d_windows, const size_t* window_bytes, uint64_t* out_counts) {
+    const u32 rb = desc->item_bytes;
+    const KeyView tkv = { 0, desc->key_bytes, TG_KEY_BYTES_BE, 0 };
+    SampleWs ws;
+    TG_TRY(sample_workspace(ctx, p, &ws));
+    SplitterDigit fn = { ws.spl, (u32)(p - 1), 0, tkv, ws.ctl, ws.lut, nullptr, nullptr };
+    auto tuples = [&](int w, ulonglong2** d_tup) -> int {
+        TG_TRY(tg_ws_get(ctx, WS_AUX, (n_shards[w] + 1) * 16, (void**)d_tup));
+        if (n_shards[w])
+            TG_LAUNCH(ctx, make_tuples_kernel, ctx->sm_count * 8, 256, 0, (const u32*)d_shards[w], (u32)n_shards[w], rb / 4,
+                      desc->key_offset, desc->key_bytes, *d_tup);
+        return TG_OK;
+    };
+    // worker w's tuples partitioned by destination into WS_AUX2 (*d_tot: its per-destination counts)
+    auto partition = [&](int w, ulonglong2** d_ptup, u32** d_tot) -> int {
+        ulonglong2* d_tup;
+        TG_TRY(tuples(w, &d_tup));
+        TG_TRY(splitters_from_slots(ctx, tkv, ws, p, w));
+        TG_TRY(tg_ws_get(ctx, WS_AUX2, (n_shards[w] + 1) * 16, (void**)d_ptup));
+        return partition_chunked<2, SplitterDigit>(ctx, d_tup, *d_ptup, n_shards[w], fn, d_tot, nullptr);
+    };
+    for (int w = 0; w < p; ++w) {
+        ulonglong2* d_tup;
+        TG_TRY(tuples(w, &d_tup));
+        TG_TRY(draw_sample_slot<2>(ctx, tkv, d_tup, n_shards[w], rng_seed, w, false, ws.slots + (size_t)w * SAMPLE_SLOT_BYTES));
+    }
+    u32* h_mat = (u32*)ctx->pinned + 16384;
+    ulonglong2* d_ptup;
+    u32* d_tot;
+    for (int w = 0; w < p; ++w) {
+        TG_TRY(partition(w, &d_ptup, &d_tot));
+        TG_CUDA(ctx, cudaMemcpyAsync(h_mat + w * p, d_tot, (size_t)p * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    TG_TRY(select_check(ctx, h_mat, p, rb, d_windows, window_bytes, out_counts));
+    if (!d_windows) return TG_OK;
+    for (int w = 0; w < p; ++w) {
+        TG_TRY(partition(w, &d_ptup, &d_tot));
+        TG_TRY(exchange_store_records(ctx, mode, true, d_shards[w], rb, d_ptup, n_shards[w], h_mat, p, w, d_windows));
+        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    }
     return TG_OK;
 }
 
@@ -843,6 +937,56 @@ int tg_sort_select(tg_ctx* ctx, const tg_key_desc* desc, const void* const* d_sh
     return desc->item_bytes == 8
                ? sort_select_impl<1>(ctx, desc, kv, d_shards, n_shards, (int)p, rng_seed, out_splitters, d_out, out_counts, out_merge_bounds)
                : sort_select_impl<2>(ctx, desc, kv, d_shards, n_shards, (int)p, rng_seed, out_splitters, d_out, out_counts, out_merge_bounds);
+}
+
+int tg_exchange_select(tg_ctx* ctx, uint32_t route, uint32_t mode, const tg_key_desc* desc, uint64_t rng_seed, uint64_t result_size,
+                       const void* const* d_shards, const size_t* n_shards, uint32_t p, void* const* d_windows,
+                       const size_t* window_bytes, uint64_t* out_counts) {
+    if (!ctx || p < 2 || p > TG_MAX_RANKS || !d_shards || !n_shards || !out_counts)
+        return tg_set_error(ctx, TG_ERR_ARG, "exchange_select: p=%u or a NULL argument", p);
+    if (route > TG_ROUTE_SPLITTERS || mode > 1) return tg_set_error(ctx, TG_ERR_ARG, "exchange_select: route %u, mode %u", route, mode);
+    for (uint32_t w = 0; w < p; ++w)
+        if (n_shards[w] && !d_shards[w]) return tg_set_error(ctx, TG_ERR_ARG, "exchange_select: shard %u is NULL", w);
+    KeyView kv = {};
+    bool records = false;
+    if (route == TG_ROUTE_SPLITTERS) {
+        if (make_key_view(desc, &kv) != TG_OK) return tg_set_error(ctx, TG_ERR_ARG, "exchange_select: unsupported descriptor");
+        records = desc->item_bytes != 8 && desc->item_bytes != 16;
+        if (records && (desc->item_bytes % 4 || desc->key_kind != TG_KEY_BYTES_BE || desc->key_bytes > 12 || desc->descending))
+            return tg_set_error(ctx, TG_ERR_ARG, "exchange_select: records need item_bytes %% 4 == 0 and an ascending byte-string key of <= 12 bytes");
+        for (uint32_t w = 0; w < p && records; ++w) {
+            if (((uintptr_t)d_shards[w]) & 3) return tg_set_error(ctx, TG_ERR_ARG, "exchange_select: records must be 4-byte aligned");
+            if (n_shards[w] >= (1u << 30)) return tg_set_error(ctx, TG_ERR_TOO_LARGE, "exchange_select: shard %u has %zu records", w, n_shards[w]);
+        }
+    }
+    if (route == TG_ROUTE_RANGE && result_size && result_size - 1 > ~0ull / p)
+        return tg_set_error(ctx, TG_ERR_ARG, "exchange_select: k * p overflows for result_size=%llu", (unsigned long long)result_size);
+    TG_CUDA(ctx, cudaSetDevice(ctx->device));
+    const int P = (int)p, M = (int)mode;
+    auto none = [](int) { return TG_OK; };
+    switch (route) {
+    case TG_ROUTE_HASH:
+        return select_items<2>(ctx, M, d_shards, n_shards, P, HashDigit{ p }, none, d_windows, window_bytes, out_counts);
+    case TG_ROUTE_MOD:
+        return select_items<2>(ctx, M, d_shards, n_shards, P, ModDigit::make(p), none, d_windows, window_bytes, out_counts);
+    case TG_ROUTE_RANGE:
+        return select_items<2>(ctx, M, d_shards, n_shards, P, RangeDigit{ result_size, p }, none, d_windows, window_bytes, out_counts);
+    default:
+        break;
+    }
+    if (records) return select_records(ctx, M, desc, rng_seed, d_shards, n_shards, P, d_windows, window_bytes, out_counts);
+    // the sample slots of every worker where the all-gather puts them, then worker w's splitters before each of its steps
+    SampleWs ws;
+    TG_TRY(sample_workspace(ctx, P, &ws));
+    for (int w = 0; w < P; ++w) {
+        const bool too_large = n_shards[w] >= (1u << 30);
+        if (desc->item_bytes == 8) TG_TRY(draw_sample_slot<1>(ctx, kv, d_shards[w], n_shards[w], rng_seed, w, too_large, ws.slots + (size_t)w * SAMPLE_SLOT_BYTES));
+        else TG_TRY(draw_sample_slot<2>(ctx, kv, d_shards[w], n_shards[w], rng_seed, w, too_large, ws.slots + (size_t)w * SAMPLE_SLOT_BYTES));
+    }
+    const SplitterDigit fn = { ws.spl, p - 1, 0, kv, ws.ctl, ws.lut, nullptr, nullptr };
+    auto prep = [&](int w) { return splitters_from_slots(ctx, kv, ws, P, w); };
+    return desc->item_bytes == 8 ? select_items<1>(ctx, M, d_shards, n_shards, P, fn, prep, d_windows, window_bytes, out_counts)
+                                 : select_items<2>(ctx, M, d_shards, n_shards, P, fn, prep, d_windows, window_bytes, out_counts);
 }
 
 int tg_sort(tg_ctx* ctx, const tg_key_desc* desc, void* d_in, size_t n_local, uint64_t rng_seed, void** out_dptr, size_t* out_n) {
