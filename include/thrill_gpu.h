@@ -26,7 +26,8 @@
  * take at most 2^30 - 1 items per worker, before and after their exchange.
  * PrefixSum, ExPrefixSum and ZipWithIndex (tg_prefix_sum, tg_zip_with_index, their _file and _select forms, tg_scan_local_total)
  * take at most 2^30 - 1 items per worker and give each worker as many items as it holds.  Sum, Min, Max and AllReduce (tg_all_reduce
- * and its _file and _select forms) take at most 2^30 - 1 items per worker.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
+ * and its _file and _select forms) and HyperLogLog (tg_hyperloglog and its _file and _select forms) take at most 2^30 - 1 items
+ * per worker.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
  ******************************************************************************/
 #ifndef THRILL_GPU_H
 #define THRILL_GPU_H
@@ -128,7 +129,8 @@ enum { TG_K_RADIX_HIST = 0, TG_K_PARTITION = 1, TG_K_MERGE = 2, TG_K_PREAGG = 3,
        TG_K_EXCHANGE = 9 /* the NCCL Alltoallv (not a kernel of ours: timed like one) */,
        TG_K_JOIN = 10 /* InnerJoin's co-rank count, offset scan and emit kernels */,
        TG_K_SCAN = 11 /* PrefixSum's tile reduce, tile prefix and scan kernels; ZipWithIndex's kernel; the actions' tile reduce
-                         and fold */, TG_K_NUM = 12 };
+                         and fold */,
+       TG_K_HLL = 12 /* HyperLogLog's hash-and-register kernel (and the register merge of tg_hyperloglog_select) */, TG_K_NUM = 13 };
 int tg_profile_enable(tg_ctx* ctx, int on);
 int tg_profile_get(tg_ctx* ctx, int kernel_class, float* out_total_ms, uint64_t* out_launches);
 /* the individual launch durations of `kernel_class` in launch order (up to `capacity`); *out_n = how many there are */
@@ -519,6 +521,47 @@ int tg_all_reduce_file(tg_ctx* ctx, const tg_scan_desc* desc, const tg_merge_inp
  * more items is TG_ERR_TOO_LARGE. */
 int tg_all_reduce_select(tg_ctx* ctx, const tg_scan_desc* desc, const void* const* d_shards, const size_t* n_shards, uint32_t p,
                          const void* initial_item, void* out_item);
+
+/* ---- HyperLogLog: the registers of a DIA's distinct-count sketch on every worker (DIA::HyperLogLog<p>, api/hyperloglog.hpp:62-72,
+ * HyperLogLogNode :26-60, core::HyperLogLogRegisters<p> core/hyperloglog.cpp) -------------------------------------------------------
+ * Stock node: every worker inserts each item, registers_.insert(x) = insert_hash(tlx::siphash(x)) (core/hyperloglog.hpp:46-50),
+ * net.AllReduce adds the workers' registers (api/hyperloglog.hpp:49-52) and result() turns them into a double.
+ * Hash: SipHash-2-4 under the fixed key bytes 0, 1, ..., 15 over the item's sizeof(T) bytes as they lie in memory
+ * (extlib/tlx/tlx/siphash.hpp:248-270): 64-bit little-endian message words, two compression rounds per word, a last word that
+ * holds the message length in its top byte, 0xff into v2 and four finalisation rounds.
+ *   item_bytes 8   uint64_t, double (hashed as its bits: +0.0 and -0.0 are two items, NaNs differ by payload)
+ *   item_bytes 16  std::pair<uint64_t, V>, V any 8-byte value: 16 message bytes, .first then .second
+ * Anything else is TG_ERR_ARG.
+ * Dense registers (core/hyperloglog.cpp:1733-1740): 2^precision registers of one byte, precision in 4..18, the set the reference
+ * instantiates (:1863-1877).  For the hash h: index = h >> (64 - precision), w = h << precision,
+ * value = (w == 0 ? 64 - precision : clz(w)) + 1, and the register is the maximum of its values; a register no item reached is
+ * 0.  The workers' registers merge by per-register max (mergeDense, :1761-1768).  Max is commutative and associative: the result
+ * is the same bytes for any sharding, worker count or timing.
+ * out_registers: 2^precision bytes on the host, the same on every rank, ALWAYS the dense register set.  The estimate is not
+ * computed here: it belongs to the stock HyperLogLogRegisters<p>::result() (:1771-1811), whose bias tables stay in the reference.
+ * GpuHyperLogLogNode builds the stock object from these bytes through its public Deserialize (:1905-1927: the format DENSE, then
+ * one uint64_t per register) and calls result() on it.
+ * Where this differs from the stock node: it starts every worker in a sparse format at precision 25 and converts to dense once
+ * the encoded sparse list outgrows 2^precision bytes (:1700-1705, :1728-1730, :1815-1859).  Its sparse -> dense conversion gives
+ * exactly the registers direct insertion gives (checked for every case of tests/golden/reference_outputs_hll.npz), so the
+ * registers here are the stock node's registers whichever format it ends in.  But if every worker and their sum are still sparse
+ * at the end, the stock result() is linear counting over 2^25 buckets (:1772-1779), while the dense registers give the dense
+ * estimate: both are valid HyperLogLog estimates of the same count, and different doubles.  That happens at small distinct counts
+ * relative to 2^precision; when the stock node converts depends on insertion order and on the duplicates in its unmerged delta
+ * set, so the boundary is not a function of the input and is not reproduced.
+ * Limits: at most 2^30 - 1 items per worker; more on any worker is TG_ERR_TOO_LARGE on every rank (a flag byte travels with the
+ * registers; a worker over the limit reads nothing).  Collective flow: the update kernel over the worker's items (none for an
+ * empty worker), with p > 1 one ncclAllReduce(ncclUint8, ncclMax) over 2^precision + 1 bytes, then one host read of them: one
+ * host round trip at any p.  No item moves between workers.  Inputs are read, never modified.  Collective. */
+/* on a device buffer */
+int tg_hyperloglog(tg_ctx* ctx, uint32_t item_bytes, uint32_t precision, const void* d_in, size_t n_local, uint8_t* out_registers);
+/* the drop-in call (GpuHyperLogLogNode::Execute): a host File (Blocks) or a device File (read in place, left intact) */
+int tg_hyperloglog_file(tg_ctx* ctx, uint32_t item_bytes, uint32_t precision, const tg_merge_input* in, uint8_t* out_registers);
+/* kernel level (1 <= p_workers <= 16 workers simulated on one device): shard w (n_shards[w] items at d_shards[w]) is worker w.
+ * Runs the update kernel per shard into the array the all-reduce would combine, then the per-register max; writes the registers
+ * every rank would get.  Shards are read, never modified; a shard of 2^30 or more items is TG_ERR_TOO_LARGE. */
+int tg_hyperloglog_select(tg_ctx* ctx, uint32_t item_bytes, uint32_t precision, const void* const* d_shards, const size_t* n_shards,
+                          uint32_t p_workers, uint8_t* out_registers);
 
 /* ---- synthetic inputs of SURVEY.md §8(d), generated on the device (bench / tests support) ------------ */
 int tg_gen_sort_uniform(tg_ctx* ctx, void* d_out, uint64_t begin, uint64_t n, uint64_t seed);

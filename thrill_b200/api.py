@@ -12,6 +12,7 @@ Mirrors (same names, argument meaning and error behaviour) the slice of thrill/a
     DIA<T>::ZipWithIndex(zip_function)     thrill/api/zip_with_index.hpp:140-152
     api::InnerJoin(l, r, key1, key2, fn)   thrill/api/inner_join.hpp:700-827
     DIA<T>::Sum / Min / Max / AllReduce    thrill/api/sum.hpp, min.hpp, max.hpp, all_reduce.hpp
+    DIA<T>::HyperLogLog<p>                 thrill/api/hyperloglog.hpp:62-72 (the registers, not the estimate)
     DIA<T>::Size / AllGather / Gather      thrill/api/size.hpp, all_gather.hpp, gather.hpp
 A DIA here holds its local shard as a host numpy array — the stand-in for a data::File whose Blocks are
 1 MiB ByteBlocks (data/byte_block.cpp:23-24, data/block_writer.hpp:405-420).  Operators hand the Blocks to the
@@ -498,6 +499,22 @@ class DIA(object):
     def Max(self, initial_value=None):
         """DIA<T>::Max (api/max.hpp): AllReduce with common::maximum, std::max(a, b) = a < b ? b : a"""
         return self.AllReduce(MaxDouble if self.items.dtype == np.float64 else MaxU64, initial_value)
+
+    def HyperLogLog(self, precision):
+        """The registers of DIA<T>::HyperLogLog<p> (api/hyperloglog.hpp): SipHash-2-4 of every item into 2^precision one-byte
+        registers, merged over the workers by max; a uint8 array, the same on every worker.  uint64, float64 (hashed as bits)
+        and KV items.  The estimate is the stock HyperLogLogRegisters<p>::result()'s to compute, not this mirror's."""
+        it = self.items
+        if it.ndim != 1 or it.dtype not in (np.uint64, np.float64, KV):
+            raise capi.ThrillGpuError("HyperLogLog: %r items are not ones the GPU path recognises" % (it.dtype,))
+        if not 4 <= precision <= 18:
+            raise capi.ThrillGpuError("HyperLogLog: precision %r is outside 4..18" % (precision,))
+        out = np.zeros(1 << precision, np.uint8)
+        blocks, nb = self._blocks(it)
+        inp = capi.MergeInput(None, C.cast(blocks, C.POINTER(capi.Block)), nb)
+        tg = self.ctx.tg
+        tg.ck(tg.L.tg_hyperloglog_file(tg.h, it.dtype.itemsize, precision, C.byref(inp), out.ctypes.data))
+        return out
 
     def Size(self):
         n = len(self.items)

@@ -36,7 +36,11 @@
 #include <thrill/api/dop_node.hpp>
 #include <thrill/common/config.hpp>
 #include <thrill/common/functional.hpp>
+#include <thrill/core/hyperloglog.hpp>
 #include <thrill/data/file.hpp>
+#include <thrill/data/serialization.hpp>
+#include <thrill/net/buffer_builder.hpp>
+#include <thrill/net/buffer_reader.hpp>
 #include <tlx/meta/call_foreach_with_index.hpp>
 #include <tlx/meta/vexpand.hpp>
 
@@ -1166,6 +1170,90 @@ private:
     size_t global_size_ = 0;
 };
 
+//! the item types HyperLogLog hashes on the GPU: 8-byte scalars (uint64_t, double: hashed as their bytes) and
+//! pair<uint64_t, V> with an 8-byte V, whose 16 bytes are .first then .second without padding
+template <typename T>
+struct HyperLogLogItem : std::integral_constant<bool, std::is_same<T, uint64_t>::value || std::is_same<T, double>::value> { };
+template <typename V>
+struct HyperLogLogItem<std::pair<uint64_t, V> >
+    : std::integral_constant<bool, sizeof(V) == 8 && sizeof(std::pair<uint64_t, V>) == 16 &&
+                             std::is_trivially_copyable<V>::value> { };
+
+//! DIA::HyperLogLog<p> (HyperLogLogNode, api/hyperloglog.hpp:26-60): the stock node protocol (a File of the parent's items, the
+//! parent's File whole through OnPreOpFile, or a parent GPU node's result in HBM) with the collective call in Execute:
+//! tg_hyperloglog_file (SipHash-2-4 and the register update on the device, one all-reduce by max over the register bytes).  The
+//! result is a stock core::HyperLogLogRegisters<p> in the dense format, built from the 2^p register bytes through its public
+//! Deserialize (core/hyperloglog.cpp:1905-1927), so result() and operator + are the reference's own.  The registers are the
+//! stock node's; where the stock node would still be sparse at the end its estimate is the sparse one, this node's the dense
+//! one (include/thrill_gpu.h, tg_hyperloglog).
+template <size_t p, typename ValueType>
+class GpuHyperLogLogNode final : public thrill::api::ActionResultNode<thrill::core::HyperLogLogRegisters<p> >, public GpuNodeBase
+{
+    using Registers = thrill::core::HyperLogLogRegisters<p>;
+    using Super = thrill::api::ActionResultNode<Registers>;
+    using Super::context_;
+
+public:
+    template <typename ParentDIA>
+    explicit GpuHyperLogLogNode(const ParentDIA& parent)
+        : Super(parent.ctx(), "GpuHyperLogLog", { parent.id() }, { parent.node() }),
+          parent_stack_empty_(ParentDIA::stack_empty) {
+        auto pre_op_fn = [this](const ValueType& input) { input_writer_.Put(input); };
+        auto lop_chain = parent.stack().push(pre_op_fn).fold();
+        parent.node()->AddChild(this, lop_chain);
+    }
+
+    void StartPreOp(size_t /* parent_index */) final { input_writer_ = input_file_.GetWriter(); }
+
+    bool OnPreOpFile(const thrill::data::File& file, size_t /* parent_index */) final {
+        if (!parent_stack_empty_) return false;
+        input_file_ = file.Copy();
+        return true;
+    }
+
+    bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes, size_t /* parent_index */) final {
+        if (!parent_stack_empty_ || item_bytes != sizeof(ValueType)) return false;
+        device_input_ = file;
+        return true;
+    }
+
+    void StopPreOp(size_t /* parent_index */) final { input_writer_.Close(); }
+
+    //! Execute (api/hyperloglog.hpp:49-52) behind one call.  Collective.
+    void Execute() final {
+        tg_ctx* c = WorkerCtx(context_);
+        std::unique_ptr<PinnedFileView> view;
+        tg_merge_input in;
+        if (device_input_) {
+            in = tg_merge_input { device_input_->get(), nullptr, 0 };
+        }
+        else {
+            view.reset(new PinnedFileView(input_file_, context_.local_worker_id()));
+            in = tg_merge_input { nullptr, view->data(), view->size() };
+        }
+        std::vector<uint8_t> regs(size_t(1) << p);
+        Check(c, tg_hyperloglog_file(c, sizeof(ValueType), p, &in, regs.data()), "tg_hyperloglog_file");
+        view.reset();
+        input_file_.Clear();
+        device_input_.reset();
+        // the serialized form of a dense object: the format, then one uint64_t per register
+        thrill::net::BufferBuilder bb;
+        bb.Put(thrill::core::HyperLogLogRegisterFormat::DENSE);
+        for (uint8_t r : regs) bb.Put(static_cast<uint64_t>(r));
+        thrill::net::BufferReader br(bb.data(), bb.size());
+        registers_ = thrill::data::Serialization<thrill::net::BufferReader, Registers>::Deserialize(br);
+    }
+
+    const Registers& result() const final { return registers_; }
+
+private:
+    const bool parent_stack_empty_;
+    thrill::data::File input_file_ { context_.GetFile(this) };
+    thrill::data::File::Writer input_writer_;
+    DeviceFilePtr device_input_;
+    Registers registers_;
+};
+
 /******************************************************************************/
 // front doors (same argument meaning as DIA<T>::Sort / DIA<T>::ReducePair)
 
@@ -1472,6 +1560,25 @@ thrill::api::Future<size_t> SizeFuture(const DIA<ValueType, Stack>& dia) {
 }
 template <typename ValueType, typename Stack>
 size_t Size(const DIA<ValueType, Stack>& dia) { return SizeFuture(dia).get(); }
+
+//! The registers of DIA<T>::HyperLogLog<p>() (api/hyperloglog.hpp:62-72) as the stock object, in the dense format: callers can
+//! add (operator +) sketches from elsewhere and call result().  uint64_t, double and pair<uint64_t, 8-byte V> items, p in 4..18.
+template <size_t p, typename ValueType, typename Stack>
+thrill::core::HyperLogLogRegisters<p> HyperLogLogRegisters(const DIA<ValueType, Stack>& dia) {
+    static_assert(HyperLogLogItem<ValueType>::value,
+                  "thrill_gpu::HyperLogLog: uint64_t, double and std::pair<uint64_t, 8-byte V> items only; "
+                  "use the stock dia.HyperLogLog<p>()");
+    static_assert(p >= 4 && p <= 18, "thrill_gpu::HyperLogLog: the precision is 4..18, as in the reference");
+    assert(dia.IsValid());
+    auto node = tlx::make_counting<GpuHyperLogLogNode<p, ValueType> >(dia);
+    node->RunScope();
+    return node->result();
+}
+//! DIA<T>::HyperLogLog<p>(): the estimate of the number of distinct items, the stock result() of the registers above
+template <size_t p, typename ValueType, typename Stack>
+double HyperLogLog(const DIA<ValueType, Stack>& dia) {
+    return HyperLogLogRegisters<p>(dia).result();
+}
 
 } // namespace thrill_gpu
 
