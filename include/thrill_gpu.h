@@ -27,7 +27,8 @@
  * PrefixSum, ExPrefixSum and ZipWithIndex (tg_prefix_sum, tg_zip_with_index, their _file and _select forms, tg_scan_local_total)
  * take at most 2^30 - 1 items per worker and give each worker as many items as it holds.  Sum, Min, Max and AllReduce (tg_all_reduce
  * and its _file and _select forms) and HyperLogLog (tg_hyperloglog and its _file and _select forms) take at most 2^30 - 1 items
- * per worker.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
+ * per worker.  Window (tg_window and its _file and _select forms) takes at most 2^30 - 1 items per worker and gives each worker at
+ * most 2^30 - 1 items.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
  ******************************************************************************/
 #ifndef THRILL_GPU_H
 #define THRILL_GPU_H
@@ -130,7 +131,8 @@ enum { TG_K_RADIX_HIST = 0, TG_K_PARTITION = 1, TG_K_MERGE = 2, TG_K_PREAGG = 3,
        TG_K_JOIN = 10 /* InnerJoin's co-rank count, offset scan and emit kernels */,
        TG_K_SCAN = 11 /* PrefixSum's tile reduce, tile prefix and scan kernels; ZipWithIndex's kernel; the actions' tile reduce
                          and fold */,
-       TG_K_HLL = 12 /* HyperLogLog's hash-and-register kernel (and the register merge of tg_hyperloglog_select) */, TG_K_NUM = 13 };
+       TG_K_HLL = 12 /* HyperLogLog's hash-and-register kernel (and the register merge of tg_hyperloglog_select) */,
+       TG_K_WINDOW = 13 /* Window's block-fold kernel */, TG_K_NUM = 14 };
 int tg_profile_enable(tg_ctx* ctx, int on);
 int tg_profile_get(tg_ctx* ctx, int kernel_class, float* out_total_ms, uint64_t* out_launches);
 /* the individual launch durations of `kernel_class` in launch order (up to `capacity`); *out_n = how many there are */
@@ -562,6 +564,58 @@ int tg_hyperloglog_file(tg_ctx* ctx, uint32_t item_bytes, uint32_t precision, co
  * every rank would get.  Shards are read, never modified; a shard of 2^30 or more items is TG_ERR_TOO_LARGE. */
 int tg_hyperloglog_select(tg_ctx* ctx, uint32_t item_bytes, uint32_t precision, const void* const* d_shards, const size_t* n_shards,
                           uint32_t p_workers, uint8_t* out_registers);
+
+/* ---- Window: folds of k consecutive items by global position (DIA::Window, api/window.hpp:284-380 and :524-564, api/dia.hpp:
+ * 1884-1935; OverlapWindowNode :140-246, DisjointWindowNode :387-503) ------------------------------------------------------------
+ * f_r = the items on the workers below r, n_r = worker r's items, N = the total, x_g = the item at global position g, and
+ * fold(x_a ... x_b) = ((x_a + x_{a+1}) + ...) + x_b, the left fold with the stock function from the window's first item
+ * (thrill_gpu::WindowFold<F> / DisjointFold<F>, thrill_b200/host/).  The index argument of the window function is not part of
+ * the output.
+ *   TG_WINDOW_FULL      Window(k, f): worker r emits fold(x_{g-k+1} ... x_g) for every g in [max(f_r, k-1), f_r + n_r), in order:
+ *                       each window goes to the worker that holds its last item (OverlapWindowNode::PushData :191-224), N - k + 1
+ *                       outputs in all (none if N < k)
+ *   TG_WINDOW_PARTIAL   Window(k, f, partial_f): the same, and the last worker (rank p - 1, even if it holds no items) appends
+ *                       fold(x_j ... x_{N-1}) for j = max(0, N-k+1) ... N-1 (:225-236)
+ *   TG_WINDOW_DISJOINT  Window(DisjointTag, k, f): worker r emits fold(x_{g-k+1} ... x_g) for every g of its range with
+ *                       (g + 1) mod k = 0 (DisjointWindowNode::PushData :447-481); if N mod k != 0 the last worker appends the
+ *                       fold of the trailing N mod k items (:483-494)
+ * The functions are the actions' set (tg_scan_desc): uint64_t with TG_OP_SUM_U64 (wraps modulo 2^64), TG_OP_MIN_U64,
+ * TG_OP_MAX_U64; double with TG_OP_SUM_F64, TG_OP_MIN_F64, TG_OP_MAX_F64; pair<uint64_t, V> with ScanSecond<F>, whose output's
+ * .first is that of the window's last item.  Other item sizes or ops are TG_ERR_ARG.
+ * Limits: 2 <= k <= 4096, otherwise TG_ERR_ARG (k = 1 is undefined in the stock node: PreOp pops an empty RingBuffer,
+ * :94-95); at most 2^30 - 1 items per worker, and at most 2^30 - 1 outputs per worker (the last one emits up to n + k - 1):
+ * otherwise TG_ERR_TOO_LARGE on every rank or on none.
+ * Exactness: integer results are exact.  Min / Max on doubles are the stock fold bit for bit: a NaN first item of a window is the
+ * output, bits included; otherwise the output is the NaN-skipping fold that keeps the left of two equal values (the sign of a zero
+ * minimum is the earlier zero's), which equals the stock left fold under any bracketing.  Double sums are bracketed by global
+ * position and k only: blocks of k items from position 0, each cut into runs of R = max(16, 2^ceil(ceil(log2 k) / 2)) items,
+ * J = ceil(k / R) runs; runs folded sequentially, run aggregates folded sequentially per block, one combine per output
+ * (tg_window.cu).  So a result has the same bits for every run, sharding, worker count and placement.  Let exact be the exact
+ * sum of the window, A the same over |x|, u = 2^-53 and gamma_D = D u / (1 - D u) with
+ *   D = min(k - 1, R + J - 1)       (15 at k = 16, 16 at k = 17, 19 at k = 64, 127 at k = 4096)
+ * the longest chain of additions a summand goes through.  While (1 + gamma_D) A < DBL_MAX, |out - exact| <= gamma_D A + u |exact|;
+ * NaN where the window holds a NaN or both infinities, the infinity where it holds one, and the sign of a zero (-0.0 exactly when
+ * every summand is -0.0) are the stock fold's.  Beyond that range a partial sum may overflow where the stock fold's do not (or
+ * the reverse), and only the bitwise reproducibility holds.  A NaN's payload is left open for sums.
+ * Collective flow: p = 1 has no collective and no host round trip (the output size follows from n_local).  With p > 1 one
+ * ncclAllGather of a fixed-size record per worker: n_local and its last min(n_local, k - 1) items, 16 + (k - 1) * item_bytes
+ * bytes rounded up to 16; then one host read of the gathered sizes, which gives the output size and the verdict on the limits.
+ * Each worker copies its halo, the k - 1 items before its first (fewer on the first workers), out of the records of ranks r - 1,
+ * r - 2, ... on the device, several when they hold fewer than k - 1 items (FlowControlChannel::Predecessor,
+ * net/flow_control_channel.hpp:644-777).  No other item moves.  Inputs are read, never modified.  Collective. */
+enum { TG_WINDOW_FULL = 0, TG_WINDOW_PARTIAL = 1, TG_WINDOW_DISJOINT = 2 };
+/* on a device buffer; *out_dptr holds *out_n items of desc->item_bytes, as for tg_sort (ctx-owned, valid until the next operator
+ * call) */
+int tg_window(tg_ctx* ctx, const tg_scan_desc* desc, const void* d_in, size_t n_local, uint32_t k, uint32_t mode,
+              void** out_dptr, size_t* out_n);
+/* the drop-in call (GpuWindowNode::Execute): a host File (Blocks) or a device File (read in place, left intact); the result is
+ * fetched with tg_fetch_output or taken with tg_output_detach */
+int tg_window_file(tg_ctx* ctx, const tg_scan_desc* desc, const tg_merge_input* in, uint32_t k, uint32_t mode, size_t* out_items);
+/* kernel level (1 <= p <= 16 workers simulated on one device): shard w (n_shards[w] items at d_shards[w]) is worker w.  Writes
+ * every worker's record into the slot the all-gather fills, then runs worker `rank`'s device path (halo and kernel); outputs as
+ * for tg_window.  Shards are read, never modified. */
+int tg_window_select(tg_ctx* ctx, const tg_scan_desc* desc, const void* const* d_shards, const size_t* n_shards, uint32_t p,
+                     uint32_t rank, uint32_t k, uint32_t mode, void** out_dptr, size_t* out_n);
 
 /* ---- synthetic inputs of SURVEY.md §8(d), generated on the device (bench / tests support) ------------ */
 int tg_gen_sort_uniform(tg_ctx* ctx, void* d_out, uint64_t begin, uint64_t n, uint64_t seed);

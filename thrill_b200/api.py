@@ -13,6 +13,7 @@ Mirrors (same names, argument meaning and error behaviour) the slice of thrill/a
     api::InnerJoin(l, r, key1, key2, fn)   thrill/api/inner_join.hpp:700-827
     DIA<T>::Sum / Min / Max / AllReduce    thrill/api/sum.hpp, min.hpp, max.hpp, all_reduce.hpp
     DIA<T>::HyperLogLog<p>                 thrill/api/hyperloglog.hpp:62-72 (the registers, not the estimate)
+    DIA<T>::Window(k, f[, partial_f])      thrill/api/window.hpp:284-380, :524-564 (the left fold of each window)
     DIA<T>::Size / AllGather / Gather      thrill/api/size.hpp, all_gather.hpp, gather.hpp
 A DIA here holds its local shard as a host numpy array — the stand-in for a data::File whose Blocks are
 1 MiB ByteBlocks (data/byte_block.cpp:23-24, data/block_writer.hpp:405-420).  Operators hand the Blocks to the
@@ -515,6 +516,23 @@ class DIA(object):
         tg = self.ctx.tg
         tg.ck(tg.L.tg_hyperloglog_file(tg.h, it.dtype.itemsize, precision, C.byref(inp), out.ctypes.data))
         return out
+
+    # ---- DIA<T>::Window (api/window.hpp:284-380, :524-564) -----------------------------------------------------------------------
+    def Window(self, window_size, fn, partial=False, disjoint=False):
+        """The left fold with fn of every window of window_size consecutive items, on the worker that holds the window's last
+        item (thrill_gpu::Window with WindowFold<F>).  partial: the last worker also emits the folds of the last min(N, k-1)
+        suffixes (Window(k, f, partial_f)).  disjoint: the windows [jk, jk+k-1], the trailing N mod k items folded on the last
+        worker (Window(DisjointTag, k, f)).  The items and functions are those of AllReduce; window_size is 2..4096."""
+        if partial and disjoint:
+            raise capi.ThrillGpuError("Window: a disjoint Window has no partial function")
+        desc = self._action_desc("Window", fn)
+        mode = capi.WINDOW_DISJOINT if disjoint else capi.WINDOW_PARTIAL if partial else capi.WINDOW_FULL
+        blocks, nb = self._blocks(self.items)
+        inp = capi.MergeInput(None, C.cast(blocks, C.POINTER(capi.Block)), nb)
+        n_out = C.c_size_t()
+        tg = self.ctx.tg
+        tg.ck(tg.L.tg_window_file(tg.h, C.byref(desc), C.byref(inp), int(window_size), mode, C.byref(n_out)))
+        return DIA(self.ctx, self._fetch(n_out.value, self.items.dtype, desc.item_bytes))
 
     def Size(self):
         n = len(self.items)

@@ -11,6 +11,8 @@
  *     thrill_gpu::GroupToIndex<Out>(dia, KeyFirst(), fn, size)    <->  DIA<T>::GroupToIndex (api/group_to_index.hpp:257)
  *     thrill_gpu::PrefixSum(dia, fn [, initial]) / ExPrefixSum    <->  DIA<T>::PrefixSum / ExPrefixSum (api/dia.hpp:1850, :1867)
  *     thrill_gpu::ZipWithIndex(dia, IndexFirst() | IndexSecond()) <->  DIA<T>::ZipWithIndex (api/zip_with_index.hpp:140)
+ *     thrill_gpu::Window(dia, k, WindowFold<F>() [, WindowFold<F>()]) <->  DIA<T>::Window(k, f[, partial_f]) (api/window.hpp:284-380)
+ *     thrill_gpu::Window(DisjointTag, dia, k, DisjointFold<F>())     <->  DIA<T>::Window(DisjointTag, k, f) (api/window.hpp:524-564)
  *     thrill_gpu::Sum / Min / Max / AllReduce (dia, ...) [Future]  <->  DIA<T>::Sum / Min / Max / AllReduce (api/sum.hpp, ...)
  *     thrill_gpu::Size(dia) / SizeFuture(dia)                     <->  DIA<T>::Size / SizeFuture (api/size.hpp)
  * Everything else of the pipeline (sources, LOps, other DOps, actions, the net/data layers) is the
@@ -36,6 +38,7 @@
 #include <thrill/api/dop_node.hpp>
 #include <thrill/common/config.hpp>
 #include <thrill/common/functional.hpp>
+#include <thrill/common/ring_buffer.hpp>
 #include <thrill/core/hyperloglog.hpp>
 #include <thrill/data/file.hpp>
 #include <thrill/data/serialization.hpp>
@@ -283,6 +286,30 @@ template <typename V, typename F>
 struct ActionDesc<std::pair<uint64_t, V>, ScanSecond<F> >
     : ActionOp<typename std::conditional<std::is_same<V, typename ScanSecond<F>::Pair::second_type>::value, V, void>::type, F>{
     static constexpr uint32_t item_bytes = 16;
+};
+//! The window functions thrill_gpu::Window recognises: the left fold with F of the window from its first item, F one of the
+//! functions of Sum / Min / Max / AllReduce (also ScanSecond<F> on pairs).  Two types, because the stock FunctionTraits needs
+//! one non-template operator (): WindowFold<F> for Window(k, f[, partial_f]) takes the RingBuffer, DisjointFold<F> for
+//! Window(DisjointTag, k, f) the vector.  The stock DIA::Window takes them as they are.
+template <typename F>
+struct WindowFold {
+    using Item = typename MemberResult<decltype(&F::operator ())>::type;
+    F fn;
+    Item operator () (size_t /* index */, const thrill::common::RingBuffer<Item>& w) const {
+        Item acc = w[0];
+        for (size_t i = 1; i < w.size(); ++i) acc = fn(acc, w[i]);
+        return acc;
+    }
+};
+template <typename F>
+struct DisjointFold {
+    using Item = typename MemberResult<decltype(&F::operator ())>::type;
+    F fn;
+    Item operator () (size_t /* index */, const std::vector<Item>& w) const {
+        Item acc = w[0];
+        for (size_t i = 1; i < w.size(); ++i) acc = fn(acc, w[i]);
+        return acc;
+    }
 };
 //! The zip functions thrill_gpu::ZipWithIndex recognises on 8-byte items: (item, index) -> pair(index, item) or pair(item, index)
 struct IndexFirst {
@@ -962,8 +989,9 @@ private:
 //! api/zip_with_index.hpp:40-128): the stock node protocol (a File of the parent's items, or the parent's File whole through
 //! OnPreOpFile) with the collective call in Execute: tg_prefix_sum_file (the all-gather of the local totals, the carry and the
 //! scan) or tg_zip_with_index_file.  The input may arrive as a device File from a parent GPU node, and the result, one item per
-//! input item on the same worker, is handed to GPU children in HBM.  zip: ZipWithIndex with index_first; otherwise PrefixSum
-//! with desc, initial and inclusive.
+//! input item on the same worker, is handed to GPU children in HBM.  zip: ZipWithIndex with index_first; window: Window
+//! (OverlapWindowNode / DisjointWindowNode, api/window.hpp:140-503) of window_k items in window_mode (TG_WINDOW_*) with desc,
+//! through tg_window_file, whose output count differs from the input's; otherwise PrefixSum with desc, initial and inclusive.
 template <typename ValueOut, typename ValueIn>
 class GpuScanNode final : public thrill::api::DOpNode<ValueOut>, public GpuNodeBase
 {
@@ -973,10 +1001,11 @@ class GpuScanNode final : public thrill::api::DOpNode<ValueOut>, public GpuNodeB
 public:
     template <typename ParentDIA>
     GpuScanNode(const ParentDIA& parent, const char* label, bool zip, const tg_scan_desc& desc, const ValueIn& initial,
-                bool inclusive, bool index_first)
+                bool inclusive, bool index_first, bool window = false, uint32_t window_k = 0,
+                uint32_t window_mode = TG_WINDOW_FULL)
         : Super(parent.ctx(), label, { parent.id() }, { parent.node() }),
-          zip_(zip), desc_(desc), initial_(initial), inclusive_(inclusive), index_first_(index_first),
-          parent_stack_empty_(ParentDIA::stack_empty) {
+          zip_(zip), desc_(desc), initial_(initial), inclusive_(inclusive), index_first_(index_first), window_(window),
+          window_k_(window_k), window_mode_(window_mode), parent_stack_empty_(ParentDIA::stack_empty) {
         auto pre_op_fn = [this](const ValueIn& input) { input_writer_.Put(input); };
         auto lop_chain = parent.stack().push(pre_op_fn).fold();
         parent.node()->AddChild(this, lop_chain);
@@ -1015,6 +1044,8 @@ public:
         size_t out_items = 0;
         if (zip_)
             Check(c, tg_zip_with_index_file(c, &in, index_first_ ? 1 : 0, &out_items), "tg_zip_with_index_file");
+        else if (window_)
+            Check(c, tg_window_file(c, &desc_, &in, window_k_, window_mode_, &out_items), "tg_window_file");
         else
             Check(c, tg_prefix_sum_file(c, &desc_, &in, &initial_, inclusive_ ? 1 : 0, &out_items), "tg_prefix_sum_file");
         view.reset();
@@ -1049,6 +1080,8 @@ private:
     const tg_scan_desc desc_;
     const ValueIn initial_;
     const bool inclusive_, index_first_;
+    const bool window_;
+    const uint32_t window_k_, window_mode_;
     const bool parent_stack_empty_;
     thrill::data::File input_file_ { context_.GetFile(this) };
     thrill::data::File::Writer input_writer_;
@@ -1060,6 +1093,8 @@ template <typename ValueType>
 using GpuPrefixSumNode = GpuScanNode<ValueType, ValueType>;
 template <typename ValueOut, typename ValueIn>
 using GpuZipWithIndexNode = GpuScanNode<ValueOut, ValueIn>;
+template <typename ValueType>
+using GpuWindowNode = GpuScanNode<ValueType, ValueType>;
 
 //! DIA::Sum / Min / Max / AllReduce (AllReduceNode, api/all_reduce.hpp:27-85): the stock node protocol (a File of the parent's
 //! items, or the parent's File whole through OnPreOpFile) with the collective call in Execute: tg_all_reduce_file (the tile
@@ -1443,6 +1478,42 @@ auto ExPrefixSum(const DIA<ValueType, Stack>& dia, const SumFunction& /* sum_fun
         tg_scan_desc { ScanDesc<ValueType, SumFunction>::item_bytes, ScanDesc<ValueType, SumFunction>::op },
         initial_element, false, false);
     return DIA<ValueType>(node);
+}
+
+//! the Window node of the recognised (item type, function) pairs: those of AllReduce.  window_size goes to tg_window_file as
+//! it is (a size past 2^32 - 1 as 2^32 - 1, also out of range), which refuses anything outside 2..4096 with TG_ERR_ARG: a die()
+//! on every rank when the node executes.
+template <typename ValueType, typename Stack, typename F>
+auto MakeWindow(const DIA<ValueType, Stack>& dia, size_t window_size, uint32_t mode, const char* label) {
+    static_assert(ActionDesc<ValueType, F>::supported && std::is_same<ValueType, typename WindowFold<F>::Item>::value,
+                  "thrill_gpu::Window: this (ValueType, window function) pair has no GPU descriptor; use the stock dia.Window");
+    assert(dia.IsValid());
+    auto node = tlx::make_counting<GpuWindowNode<ValueType> >(
+        dia, label, false, tg_scan_desc { ActionDesc<ValueType, F>::item_bytes, ActionDesc<ValueType, F>::op }, ValueType(),
+        false, false, true, static_cast<uint32_t>(window_size > 0xffffffffu ? 0xffffffffu : window_size), mode);
+    return DIA<ValueType>(node);
+}
+
+//! DIA<T>::Window(k, window_function) (api/window.hpp:284-324) with WindowFold<F>: worker r emits the fold of x_{g-k+1} ... x_g
+//! for every g it holds with g >= k - 1 (include/thrill_gpu.h, tg_window).  Double sums are bracketed by global position and k:
+//! the same bits for every sharding, within the bound the header states.
+template <typename ValueType, typename Stack, typename F>
+auto Window(const DIA<ValueType, Stack>& dia, size_t window_size, const WindowFold<F>& /* window_function */) {
+    return MakeWindow<ValueType, Stack, F>(dia, window_size, TG_WINDOW_FULL, "GpuWindow");
+}
+//! DIA<T>::Window(k, window_function, partial_window_function) (api/window.hpp:326-380): the same, and the last worker appends
+//! the folds of the last min(N, k - 1) suffixes
+template <typename ValueType, typename Stack, typename F>
+auto Window(const DIA<ValueType, Stack>& dia, size_t window_size, const WindowFold<F>& /* window_function */,
+            const WindowFold<F>& /* partial_window_function */) {
+    return MakeWindow<ValueType, Stack, F>(dia, window_size, TG_WINDOW_PARTIAL, "GpuWindow");
+}
+//! DIA<T>::Window(DisjointTag, k, window_function) (api/window.hpp:524-564) with DisjointFold<F>: the folds of the blocks
+//! [jk, jk + k - 1], each on the worker holding its last item, and of the trailing N mod k items on the last worker
+template <typename ValueType, typename Stack, typename F>
+auto Window(const struct thrill::api::DisjointTag& /* tag */, const DIA<ValueType, Stack>& dia, size_t window_size,
+            const DisjointFold<F>& /* window_function */) {
+    return MakeWindow<ValueType, Stack, F>(dia, window_size, TG_WINDOW_DISJOINT, "GpuDisjointWindow");
 }
 
 //! DIA<T>::ZipWithIndex(zip_function) (api/zip_with_index.hpp:140-152) of 8-byte trivially copyable items with
