@@ -28,7 +28,8 @@
  * take at most 2^30 - 1 items per worker and give each worker as many items as it holds.  Sum, Min, Max and AllReduce (tg_all_reduce
  * and its _file and _select forms) and HyperLogLog (tg_hyperloglog and its _file and _select forms) take at most 2^30 - 1 items
  * per worker.  Window (tg_window and its _file and _select forms) takes at most 2^30 - 1 items per worker and gives each worker at
- * most 2^30 - 1 items.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
+ * most 2^30 - 1 items.  Sample and BernoulliSample (tg_sample, tg_bernoulli_sample and their _file and _select forms) take at most
+ * 2^30 - 1 items per worker.  The collective operators return TG_ERR_TOO_LARGE on every rank or on none.
  ******************************************************************************/
 #ifndef THRILL_GPU_H
 #define THRILL_GPU_H
@@ -132,7 +133,9 @@ enum { TG_K_RADIX_HIST = 0, TG_K_PARTITION = 1, TG_K_MERGE = 2, TG_K_PREAGG = 3,
        TG_K_SCAN = 11 /* PrefixSum's tile reduce, tile prefix and scan kernels; ZipWithIndex's kernel; the actions' tile reduce
                          and fold */,
        TG_K_HLL = 12 /* HyperLogLog's hash-and-register kernel (and the register merge of tg_hyperloglog_select) */,
-       TG_K_WINDOW = 13 /* Window's block-fold kernel */, TG_K_NUM = 14 };
+       TG_K_WINDOW = 13 /* Window's block-fold kernel */,
+       TG_K_SAMPLE = 14 /* Sample's and BernoulliSample's histogram, candidate, digit-pick, count, tile-scan and write kernels */,
+       TG_K_NUM = 15 };
 int tg_profile_enable(tg_ctx* ctx, int on);
 int tg_profile_get(tg_ctx* ctx, int kernel_class, float* out_total_ms, uint64_t* out_launches);
 /* the individual launch durations of `kernel_class` in launch order (up to `capacity`); *out_n = how many there are */
@@ -616,6 +619,62 @@ int tg_window_file(tg_ctx* ctx, const tg_scan_desc* desc, const tg_merge_input* 
  * for tg_window.  Shards are read, never modified. */
 int tg_window_select(tg_ctx* ctx, const tg_scan_desc* desc, const void* const* d_shards, const size_t* n_shards, uint32_t p,
                      uint32_t rank, uint32_t k, uint32_t mode, void** out_dptr, size_t* out_n);
+
+/* ---- Sample / BernoulliSample: uniform samples without replacement by global position (DIA::Sample, SampleNode
+ * api/sample.hpp:37-140; DIA::BernoulliSample, api/bernoulli_sample.hpp:27-77) ----------------------------------------------------
+ * f_r = the items on the workers below r, N = the total.  Global position g gets the 64-bit key
+ *   key(seed, g) = mix(mix(seed) + (g + 1) * 0x9e3779b97f4a7c15)   (mod 2^64)
+ * with mix(z) the SplitMix64 output function: z ^= z >> 30; z *= 0xbf58476d1ce4e5b9; z ^= z >> 27; z *= 0x94d049bb133111eb;
+ * z ^= z >> 31.  mix is a bijection and the increment is odd, so distinct positions have distinct keys: there are no ties.  (The
+ * outer mix(seed) keeps seeds that differ by a multiple of the increment, such as the Python Context's successive seeds, from
+ * drawing shifted copies of one key stream.)
+ *   Sample(s)            s >= N keeps every item (the stock underfull branch, sample.hpp:91-98); s = 0 keeps none; otherwise
+ *                        position g is kept iff key(seed, g) <= K, K the s-th smallest key of the N positions: exactly s items
+ *   BernoulliSample(p)   position g is kept iff (key(seed, g) >> 11) < ceil(p * 2^53), i.e. u < p for the 53-bit uniform
+ *                        u = (key >> 11) * 2^-53; p = 0 keeps nothing and p = 1 everything; p that is NaN or outside [0, 1] is
+ *                        TG_ERR_ARG (the stock node asserts)
+ * Both are uniform, as the stock operators are: every s-subset of the positions is equally likely under a uniform seed, and every
+ * position is kept independently with probability p.  Given the seed, the result is the same items for every sharding and worker
+ * count, and finding which positions to keep reads no item.
+ * Placement and order: kept items stay on their worker, in input order.  For BernoulliSample this is the stock order.  The stock
+ * Sample leaves its reservoir's internal (random) order; Thrill promises no order, and input order is one of the outcomes it
+ * allows.  Each worker's count has the stock distribution (multivariate hypergeometric for Sample).  Sampling with replacement
+ * is not built.
+ * Seed: rank 0's seed is the operator's seed, the other ranks' seed arguments are ignored (the stock node broadcasts rank 0's
+ * draw, sample.hpp:101-108); it travels in the all-gathered record, and so do s or the bits of p: if they differ between ranks the
+ * result is TG_ERR_ARG on every rank.
+ * Items: item_bytes a multiple of 4 from 4 to 256 (u64, double, pairs, the join's tuples, 100-byte records, points of up to 32
+ * doubles), copied as bytes; anything else is TG_ERR_ARG.  Limits: at most 2^30 - 1 items per worker and 16 workers; more items on
+ * any worker is TG_ERR_TOO_LARGE on every rank or on none, decided from the gathered sizes before any item is read.
+ * Collective flow: with p > 1 one ncclAllGather of a 32-byte record per worker (n_local, seed, s or the bits of p) and one host read
+ * of the records, which gives the worker's global offset and N.  Sample with 0 < s < N then finds K on the device, one digit per
+ * round (12, 12, 12, 12, 12, 4 bits), each round a histogram summed by one ncclAllReduce of at most 4096 u64 and a one-CTA pick, with
+ * no host synchronisation between rounds; the first two rounds hash every local position, the others only the keys of the chosen
+ * top-12-bit bin.  Both operators then count the kept positions per tile, scan the counts, read the worker's output count (one
+ * host read) and write the kept items in order, loading only their bytes.  With p = 1 there is no collective, and the host read of
+ * the output count is the only round trip: none for Sample (it keeps s), none when nothing or everything is kept.  Inputs are read,
+ * never modified.  Collective. */
+/* on a device buffer; *out_dptr holds *out_n items of item_bytes, as for tg_sort (ctx-owned, valid until the next operator call) */
+int tg_sample(tg_ctx* ctx, uint32_t item_bytes, const void* d_in, size_t n_local, uint64_t sample_size, uint64_t seed,
+              void** out_dptr, size_t* out_n);
+int tg_bernoulli_sample(tg_ctx* ctx, uint32_t item_bytes, const void* d_in, size_t n_local, double p, uint64_t seed,
+                        void** out_dptr, size_t* out_n);
+/* the drop-in calls (GpuSampleNode::Execute): a host File (Blocks) or a device File (read in place, left intact); the result is
+ * fetched with tg_fetch_output or taken with tg_output_detach */
+int tg_sample_file(tg_ctx* ctx, uint32_t item_bytes, const tg_merge_input* in, uint64_t sample_size, uint64_t seed,
+                   size_t* out_items);
+int tg_bernoulli_sample_file(tg_ctx* ctx, uint32_t item_bytes, const tg_merge_input* in, double p, uint64_t seed,
+                             size_t* out_items);
+/* kernel level (1 <= p_workers <= 16 workers simulated on one device): shard w (n_shards[w] items at d_shards[w]) is worker w, with
+ * the sample size sample_sizes[w] (or probability ps[w]) and seed seeds[w] it would pass.  Runs worker `rank`'s device path with
+ * the records of every worker in place of the all-gather, and every worker's histogram kernels into one histogram in place of
+ * the all-reduce; outputs as for tg_sample.  The verdict on the limits and arguments comes before any shard is read.  Shards are
+ * read, never modified. */
+int tg_sample_select(tg_ctx* ctx, uint32_t item_bytes, const void* const* d_shards, const size_t* n_shards, uint32_t p_workers,
+                     uint32_t rank, const uint64_t* sample_sizes, const uint64_t* seeds, void** out_dptr, size_t* out_n);
+int tg_bernoulli_sample_select(tg_ctx* ctx, uint32_t item_bytes, const void* const* d_shards, const size_t* n_shards,
+                               uint32_t p_workers, uint32_t rank, const double* ps, const uint64_t* seeds, void** out_dptr,
+                               size_t* out_n);
 
 /* ---- synthetic inputs of SURVEY.md §8(d), generated on the device (bench / tests support) ------------ */
 int tg_gen_sort_uniform(tg_ctx* ctx, void* d_out, uint64_t begin, uint64_t n, uint64_t seed);

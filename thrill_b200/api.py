@@ -14,6 +14,7 @@ Mirrors (same names, argument meaning and error behaviour) the slice of thrill/a
     DIA<T>::Sum / Min / Max / AllReduce    thrill/api/sum.hpp, min.hpp, max.hpp, all_reduce.hpp
     DIA<T>::HyperLogLog<p>                 thrill/api/hyperloglog.hpp:62-72 (the registers, not the estimate)
     DIA<T>::Window(k, f[, partial_f])      thrill/api/window.hpp:284-380, :524-564 (the left fold of each window)
+    DIA<T>::Sample / BernoulliSample       thrill/api/sample.hpp:37-140, bernoulli_sample.hpp:27-77 (by global position)
     DIA<T>::Size / AllGather / Gather      thrill/api/size.hpp, all_gather.hpp, gather.hpp
 A DIA here holds its local shard as a host numpy array — the stand-in for a data::File whose Blocks are
 1 MiB ByteBlocks (data/byte_block.cpp:23-24, data/block_writer.hpp:405-420).  Operators hand the Blocks to the
@@ -533,6 +534,32 @@ class DIA(object):
         tg = self.ctx.tg
         tg.ck(tg.L.tg_window_file(tg.h, C.byref(desc), C.byref(inp), int(window_size), mode, C.byref(n_out)))
         return DIA(self.ctx, self._fetch(n_out.value, self.items.dtype, desc.item_bytes))
+
+    # ---- DIA<T>::Sample / BernoulliSample (api/sample.hpp:37-140, api/bernoulli_sample.hpp:27-77) ----------------------------------
+    def _sample(self, what, call, param, seed):
+        it = self.items
+        ib = it.dtype.itemsize * (it.shape[1] if it.ndim == 2 else 1)
+        if it.ndim not in (1, 2) or ib % 4 or not 4 <= ib <= 256:
+            raise capi.ThrillGpuError("%s: %d-byte items (a multiple of 4 bytes from 4 to 256)" % (what, ib))
+        seed = self.ctx._next_seed() if seed is None else int(seed) % (1 << 64)
+        blocks, nb = self._blocks(it)
+        inp = capi.MergeInput(None, C.cast(blocks, C.POINTER(capi.Block)), nb)
+        n_out = C.c_size_t()
+        tg = self.ctx.tg
+        tg.ck(call(tg.h, ib, C.byref(inp), param, seed, C.byref(n_out)))
+        out = self._fetch(n_out.value, None if it.ndim == 2 else it.dtype, ib)
+        return DIA(self.ctx, out.view(it.dtype) if it.ndim == 2 else out)
+
+    def Sample(self, sample_size, seed=None):
+        """A uniform sample of min(sample_size, N) items without replacement: the positions with the sample_size smallest keys
+        key(seed, g) (include/thrill_gpu.h), each kept item on its worker in input order.  Rank 0's seed wins; without one every
+        rank draws ctx._next_seed()."""
+        return self._sample("Sample", self.ctx.tg.L.tg_sample_file, int(sample_size), seed)
+
+    def BernoulliSample(self, p, seed=None):
+        """Every item kept independently with probability p: position g iff (key(seed, g) >> 11) < ceil(p * 2^53), kept items on
+        their worker in input order.  p outside [0, 1] or NaN is an error."""
+        return self._sample("BernoulliSample", self.ctx.tg.L.tg_bernoulli_sample_file, float(p), seed)
 
     def Size(self):
         n = len(self.items)

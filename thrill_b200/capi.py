@@ -13,7 +13,7 @@ TG_OK = 0
 KEY_UINT_LE, KEY_BYTES_BE = 0, 1
 OP_SUM_F64, OP_SUM_U64, OP_MIN_U64, OP_MAX_U64, OP_MIN_F64, OP_MAX_F64, OP_FIRST = range(7)
 K_RADIX_HIST, K_PARTITION, K_MERGE, K_PREAGG, K_AGGREGATE, K_COMPACT, K_OTHER, K_FIXUP, K_SEGCOUNT, K_EXCHANGE, K_JOIN, K_SCAN, K_HLL, \
-    K_WINDOW = range(14)
+    K_WINDOW, K_SAMPLE = range(15)
 WINDOW_FULL, WINDOW_PARTIAL, WINDOW_DISJOINT = range(3)
 JOIN_KEY_VALUES, JOIN_VALUES = 0, 1
 ROUTE_HASH, ROUTE_MOD, ROUTE_RANGE, ROUTE_SPLITTERS = range(4)
@@ -148,6 +148,12 @@ SYMBOLS = [
     ("tg_window", _i, [_vp, _P(ScanDesc), _vp, _sz, _u32, _u32, _P(_vp), _P(_sz)]),
     ("tg_window_file", _i, [_vp, _P(ScanDesc), _P(MergeInput), _u32, _u32, _P(_sz)]),
     ("tg_window_select", _i, [_vp, _P(ScanDesc), _P(_vp), _P(_sz), _u32, _u32, _u32, _u32, _P(_vp), _P(_sz)]),
+    ("tg_sample", _i, [_vp, _u32, _vp, _sz, _u64, _u64, _P(_vp), _P(_sz)]),
+    ("tg_bernoulli_sample", _i, [_vp, _u32, _vp, _sz, C.c_double, _u64, _P(_vp), _P(_sz)]),
+    ("tg_sample_file", _i, [_vp, _u32, _P(MergeInput), _u64, _u64, _P(_sz)]),
+    ("tg_bernoulli_sample_file", _i, [_vp, _u32, _P(MergeInput), C.c_double, _u64, _P(_sz)]),
+    ("tg_sample_select", _i, [_vp, _u32, _P(_vp), _P(_sz), _u32, _u32, _P(_u64), _P(_u64), _P(_vp), _P(_sz)]),
+    ("tg_bernoulli_sample_select", _i, [_vp, _u32, _P(_vp), _P(_sz), _u32, _u32, _P(C.c_double), _P(_u64), _P(_vp), _P(_sz)]),
     ("tg_transfer_bytes", _i, [_vp, _P(_u64), _P(_u64)]),
     ("tg_gen_sort_uniform", _i, [_vp, _vp, _u64, _u64, _u64]),
     ("tg_gen_reduce_uniform", _i, [_vp, _vp, _u64, _u64, _u64, _u64, _i]),

@@ -1096,6 +1096,104 @@ using GpuZipWithIndexNode = GpuScanNode<ValueOut, ValueIn>;
 template <typename ValueType>
 using GpuWindowNode = GpuScanNode<ValueType, ValueType>;
 
+//! DIA::Sample (SampleNode, api/sample.hpp:37-140) and DIA::BernoulliSample (api/bernoulli_sample.hpp:27-77) by global position:
+//! the stock node protocol (a File of the parent's items, or the parent's File whole through OnPreOpFile) with the collective call
+//! in Execute: tg_sample_file / tg_bernoulli_sample_file (one all-gather of the workers' records, the selection of the s-th
+//! smallest key on the device, the compaction).  The input may arrive as a device File from a parent GPU node; the kept items stay
+//! on their worker in input order and are handed to GPU children in HBM.  bernoulli: keep each item with probability p, else a
+//! sample of sample_size items.  Rank 0's seed wins.
+template <typename ValueType>
+class GpuSampleNode final : public thrill::api::DOpNode<ValueType>, public GpuNodeBase
+{
+    using Super = thrill::api::DOpNode<ValueType>;
+    using Super::context_;
+
+public:
+    template <typename ParentDIA>
+    GpuSampleNode(const ParentDIA& parent, const char* label, bool bernoulli, uint64_t sample_size, double p, uint64_t seed)
+        : Super(parent.ctx(), label, { parent.id() }, { parent.node() }),
+          bernoulli_(bernoulli), sample_size_(sample_size), p_(p), seed_(seed), parent_stack_empty_(ParentDIA::stack_empty) {
+        auto pre_op_fn = [this](const ValueType& input) { input_writer_.Put(input); };
+        auto lop_chain = parent.stack().push(pre_op_fn).fold();
+        parent.node()->AddChild(this, lop_chain);
+    }
+
+    void StartPreOp(size_t /* parent_index */) final { input_writer_ = input_file_.GetWriter(); }
+
+    bool OnPreOpFile(const thrill::data::File& file, size_t /* parent_index */) final {
+        if (!parent_stack_empty_) return false;
+        input_file_ = file.Copy();
+        return true;
+    }
+
+    bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes, size_t /* parent_index */) final {
+        if (!parent_stack_empty_ || item_bytes != sizeof(ValueType)) return false;
+        device_input_ = file;
+        return true;
+    }
+
+    void StopPreOp(size_t /* parent_index */) final { input_writer_.Close(); }
+
+    DIAMemUse ExecuteMemUse() final { return DIAMemUse::Max(); }
+
+    //! Execute (sample.hpp:72-124) and the draw of PushData (:126-140) behind one call.  Collective.
+    void Execute() final {
+        tg_ctx* c = WorkerCtx(context_);
+        std::unique_ptr<PinnedFileView> view;
+        tg_merge_input in;
+        if (device_input_) {
+            in = tg_merge_input { device_input_->get(), nullptr, 0 };
+        }
+        else {
+            view.reset(new PinnedFileView(input_file_, context_.local_worker_id()));
+            in = tg_merge_input { nullptr, view->data(), view->size() };
+        }
+        size_t out_items = 0;
+        const uint32_t ib = sizeof(ValueType);
+        if (bernoulli_)
+            Check(c, tg_bernoulli_sample_file(c, ib, &in, p_, seed_, &out_items), "tg_bernoulli_sample_file");
+        else
+            Check(c, tg_sample_file(c, ib, &in, sample_size_, seed_, &out_items), "tg_sample_file");
+        view.reset();
+        input_file_.Clear();
+        device_input_.reset();
+        tg_dev_file f;
+        Check(c, tg_output_detach(c, &f), "tg_output_detach");
+        device_result_ = std::make_shared<DeviceFile>(c, f);
+        have_host_file_ = false;
+    }
+
+    DIAMemUse PushDataMemUse() final { return 0; }
+
+    void PushData(bool consume) final {
+        if (device_result_ && AllChildrenAreGpuNodes(*this)) {
+            bool all = true;
+            for (const auto& ch : this->children_)
+                all = dynamic_cast<GpuNodeBase*>(ch.node)->OnPreOpDeviceFile(device_result_, sizeof(ValueType), ch.parent_index) && all;
+            if (all) return;
+        }
+        if (!have_host_file_) {
+            FetchDeviceFileIntoFile(WorkerCtx(context_), context_, *device_result_, sizeof(ValueType), result_file_);
+            have_host_file_ = true;
+        }
+        this->PushFile(result_file_, consume);
+    }
+
+    void Dispose() final { result_file_.Clear(); device_result_.reset(); have_host_file_ = false; }
+
+private:
+    const bool bernoulli_;
+    const uint64_t sample_size_;
+    const double p_;
+    const uint64_t seed_;
+    const bool parent_stack_empty_;
+    thrill::data::File input_file_ { context_.GetFile(this) };
+    thrill::data::File::Writer input_writer_;
+    thrill::data::File result_file_ { context_.GetFile(this) };
+    DeviceFilePtr device_input_, device_result_;
+    bool have_host_file_ = false;
+};
+
 //! DIA::Sum / Min / Max / AllReduce (AllReduceNode, api/all_reduce.hpp:27-85): the stock node protocol (a File of the parent's
 //! items, or the parent's File whole through OnPreOpFile) with the collective call in Execute: tg_all_reduce_file (the tile
 //! reduce, one all-gather of the workers' records, the fold on the device).  A parent GPU node hands its result over in HBM, so
@@ -1514,6 +1612,47 @@ template <typename ValueType, typename Stack, typename F>
 auto Window(const struct thrill::api::DisjointTag& /* tag */, const DIA<ValueType, Stack>& dia, size_t window_size,
             const DisjointFold<F>& /* window_function */) {
     return MakeWindow<ValueType, Stack, F>(dia, window_size, TG_WINDOW_DISJOINT, "GpuDisjointWindow");
+}
+
+//! the Sample / BernoulliSample node of trivially copyable items of 4..256 bytes, a multiple of 4 (copied as bytes)
+template <typename ValueType, typename Stack>
+auto MakeSample(const DIA<ValueType, Stack>& dia, bool bernoulli, uint64_t sample_size, double p, uint64_t seed) {
+    static_assert(std::is_trivially_copyable<ValueType>::value && sizeof(ValueType) % 4 == 0 && sizeof(ValueType) >= 4 &&
+                  sizeof(ValueType) <= 256,
+                  "thrill_gpu::Sample / BernoulliSample: items must be trivially copyable, of 4..256 bytes, a multiple of 4; use "
+                  "the stock dia.Sample / dia.BernoulliSample");
+    assert(dia.IsValid());
+    auto node = tlx::make_counting<GpuSampleNode<ValueType> >(dia, bernoulli ? "GpuBernoulliSample" : "GpuSample", bernoulli,
+                                                              sample_size, p, seed);
+    return DIA<ValueType>(node);
+}
+
+//! a 64-bit seed from the worker's generator (rank 0's wins in the library)
+inline uint64_t DrawSeed(thrill::api::Context& ctx) {
+    const uint64_t hi = ctx.rng_();
+    return (hi << 32) ^ ctx.rng_();
+}
+
+//! DIA<T>::Sample(sample_size) (api/sample.hpp:150-165): min(sample_size, N) items drawn uniformly without replacement, the
+//! positions with the smallest keys key(seed, g) (include/thrill_gpu.h, tg_sample).  Kept items stay on their worker, in input
+//! order (one of the orders the stock node allows).  Without a seed, each worker draws one from context().rng_.
+template <typename ValueType, typename Stack>
+auto Sample(const DIA<ValueType, Stack>& dia, size_t sample_size) {
+    return MakeSample(dia, false, sample_size, 0.0, DrawSeed(dia.ctx()));
+}
+template <typename ValueType, typename Stack>
+auto Sample(const DIA<ValueType, Stack>& dia, size_t sample_size, uint64_t seed) {
+    return MakeSample(dia, false, sample_size, 0.0, seed);
+}
+//! DIA<T>::BernoulliSample(p) (api/bernoulli_sample.hpp:89-106): every item kept independently with probability p, in input
+//! order.  p that is NaN or outside [0, 1] is a die() on every rank when the node executes.
+template <typename ValueType, typename Stack>
+auto BernoulliSample(const DIA<ValueType, Stack>& dia, double p) {
+    return MakeSample(dia, true, 0, p, DrawSeed(dia.ctx()));
+}
+template <typename ValueType, typename Stack>
+auto BernoulliSample(const DIA<ValueType, Stack>& dia, double p, uint64_t seed) {
+    return MakeSample(dia, true, 0, p, seed);
 }
 
 //! DIA<T>::ZipWithIndex(zip_function) (api/zip_with_index.hpp:140-152) of 8-byte trivially copyable items with
