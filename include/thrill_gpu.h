@@ -20,8 +20,8 @@
  * tg_reduce_to_index and their _file / _dev forms) takes at most 2^30 - 1 items per call and worker (n_local), and a worker receives at most 2^30 - 1
  * items in an exchange (tg_exchange_select included): the partition passes count in 30-bit fields.  ReduceToIndex gives each worker fewer than 2^31
  * indices of the result.  Merge (tg_merge and its forms) takes at most 2^30 - 1 items in a worker's k inputs together, and gives
- * each worker at most 2^30 - 1 items of the result; it merges 2..16 inputs of 8- or 16-byte items.  InnerJoin (tg_inner_join
- * and its _file form) takes at most 2^30 - 1 items per worker and side, before and after its exchange, and gives each worker at
+ * each worker at most 2^30 - 1 items of the result; it merges 2..16 inputs of 8- or 16-byte items.  InnerJoin (tg_inner_join,
+ * tg_inner_join_records and their _file forms) takes at most 2^30 - 1 items per worker and side, before and after its exchange, and gives each worker at
  * most 2^30 - 1 items of the result.  GroupByKey and GroupToIndex (tg_group_by_key, tg_group_to_index and their _file forms)
  * take at most 2^30 - 1 items per worker, before and after their exchange.
  * PrefixSum, ExPrefixSum and ZipWithIndex (tg_prefix_sum, tg_zip_with_index, their _file and _select forms, tg_scan_local_total)
@@ -129,7 +129,7 @@ uint64_t tg_hot_records(const tg_ctx* ctx);
 enum { TG_K_RADIX_HIST = 0, TG_K_PARTITION = 1, TG_K_MERGE = 2, TG_K_PREAGG = 3, TG_K_AGGREGATE = 4,
        TG_K_COMPACT = 5, TG_K_OTHER = 6, TG_K_FIXUP = 7, TG_K_SEGCOUNT = 8,
        TG_K_EXCHANGE = 9 /* the NCCL Alltoallv (not a kernel of ours: timed like one) */,
-       TG_K_JOIN = 10 /* InnerJoin's co-rank count, offset scan and emit kernels */,
+       TG_K_JOIN = 10 /* InnerJoin's co-rank count, offset scan and emit kernels (pairs and records) */,
        TG_K_SCAN = 11 /* PrefixSum's tile reduce, tile prefix and scan kernels; ZipWithIndex's kernel; the actions' tile reduce
                          and fold */,
        TG_K_HLL = 12 /* HyperLogLog's hash-and-register kernel (and the register merge of tg_hyperloglog_select) */,
@@ -390,6 +390,51 @@ int tg_inner_join(tg_ctx* ctx, const tg_join_desc* desc, const void* d_left, siz
  * result is fetched with tg_fetch_output or taken with tg_output_detach (item_bytes 24 or 16) */
 int tg_inner_join_file(tg_ctx* ctx, const tg_join_desc* desc, const tg_merge_input* left, const tg_merge_input* right,
                        size_t* out_items);
+
+/* ---- InnerJoin on records: DIA<L> ⋈ DIA<R> of fixed-size PODs on an unsigned integer key field (api::InnerJoin,
+ * api/inner_join.hpp:700-827; JoinNode :61-481) ---------------------------------------------------------------------------------
+ * Items: each side a trivially copyable T serialized as its raw sizeof(T) bytes (data/serialization.hpp, the is_pod case), or a
+ * pair<uint64_t, V> with V POD (member-wise: 8 + sizeof(V) bytes); 4 <= size <= 1024 and size % 4 == 0, the two sides' sizes may
+ * differ.  Key: an unsigned little-endian integer of key_bytes = 1..8 bytes at any byte offset inside the item (no alignment
+ * needed); both sides' keys are compared as zero-extended u64.  Every pair (l, r) with equal keys gives one output item, the
+ * join function thrill_gpu::JoinPair: std::pair<L, R>, serialized as left_bytes + right_bytes bytes, the left item's bytes then
+ * the right item's, every byte a bit copy (padding and NaN payloads included).
+ * Placement: worker Hash128to64(0, key) % p owns a key, as in tg_inner_join (a 16-byte pair lands on the same worker through
+ * either entry point).  The reference's JoinNode exchanges and sorts whole records on the host; here each side's records go
+ * through 16-byte tuples {key, position}: with p > 1 the tuples are partitioned by the owner and the records follow them into
+ * the owners' windows (each record crosses NVLink once), then per worker the tuples of the received records are stably sorted by
+ * the key, the co-rank count, the offset scan and the output-stationary emit run as in tg_inner_join, and the emit copies each
+ * output's two records from where they lie (an input is read once, at the emit, with p = 1).
+ * Order within a worker: ascending key, then the left item's global position, then the right item's — one of the outcomes the
+ * reference allows (it places by std::hash % p and sorts with std::sort, so comparisons with it are on the multiset).
+ * Limits: 2^30 or more items of a side on a worker, before or after the exchange, or an output of 2^30 or more items on any worker
+ * (agreed on by an all-reduce before output memory is allocated), is TG_ERR_TOO_LARGE on every rank.  TG_ERR_ARG: a size of 0,
+ * not a multiple of 4 or over 1024, key_bytes 0 or over 8, a key that does not lie inside its item, records not 4-byte aligned,
+ * a host File whose byte count is not a multiple of its item size, a device File whose item_bytes differs from the descriptor.
+ * Inputs are read, never modified; an input may be the un-detached result of an earlier operator on this ctx (it is copied out
+ * of the join's way first).  An empty side gives an empty result.  Host round trips: with p = 1 one (the output size), with
+ * p > 1 three (the two count matrices and the output-size all-reduce).  Collective. */
+typedef struct {
+    uint32_t left_bytes, right_bytes;               /* item sizes */
+    uint32_t left_key_offset, left_key_bytes;       /* the key field of a left item */
+    uint32_t right_key_offset, right_key_bytes;     /* ... of a right item */
+} tg_join_records_desc;
+/* device buffers; *out_dptr as for tg_sort (ctx-owned, valid until the next operator call).  Collective. */
+int tg_inner_join_records(tg_ctx* ctx, const tg_join_records_desc* desc, const void* d_left, size_t n_left, const void* d_right,
+                          size_t n_right, void** out_dptr, size_t* out_n);
+/* the drop-in call (GpuJoinNode<..., tg_join_records_desc>::Execute): each side a host File or a device File (read in place, left intact); the
+ * result (items of left_bytes + right_bytes) is fetched with tg_fetch_output or taken with tg_output_detach */
+int tg_inner_join_records_file(tg_ctx* ctx, const tg_join_records_desc* desc, const tg_merge_input* left,
+                               const tg_merge_input* right, size_t* out_items);
+/* The records' exchange of the join for p simulated workers on one device (1 <= p <= 16), as tg_exchange_select does for its
+ * routes: shard w (n_shards[w] records of item_bytes, key as in the descriptor) is worker w's input; window d receives the records
+ * every worker sends to worker Hash128to64(0, key) % p, grouped by source worker in rank order, each group in the sender's input
+ * order.  mode 1 stores the records straight into the windows, mode 0 goes through the local send buffer and device copies of
+ * what ncclSend / ncclRecv move.  out_counts, TG_ERR_TOO_LARGE, d_windows == NULL and the window sizes as in tg_exchange_select.
+ * tg_inner_join_records at p = 1 on each window gives that worker's result. */
+int tg_exchange_records_select(tg_ctx* ctx, uint32_t mode, uint32_t item_bytes, uint32_t key_offset, uint32_t key_bytes,
+                               const void* const* d_shards, const size_t* n_shards, uint32_t p, void* const* d_windows,
+                               const size_t* window_bytes, uint64_t* out_counts);
 
 /* ---- GroupByKey / GroupToIndex: a DIA<pair<u64, V>> grouped by .first (DIA::GroupByKey, api/group_by_key.hpp:46-428;
  * DIA::GroupToIndex, api/group_to_index.hpp:36-290) ---------------------------------------------------------------------------

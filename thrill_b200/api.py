@@ -10,7 +10,7 @@ Mirrors (same names, argument meaning and error behaviour) the slice of thrill/a
     DIA<T>::GroupByKey / GroupToIndex      thrill/api/group_by_key.hpp:419-428, group_to_index.hpp:257-290
     DIA<T>::PrefixSum / ExPrefixSum        thrill/api/dia.hpp:1850, :1867 (api/prefix_sum.hpp, ex_prefix_sum.hpp)
     DIA<T>::ZipWithIndex(zip_function)     thrill/api/zip_with_index.hpp:140-152
-    api::InnerJoin(l, r, key1, key2, fn)   thrill/api/inner_join.hpp:700-827
+    api::InnerJoin(l, r, key1, key2, fn)   thrill/api/inner_join.hpp:700-827 (pairs on .first; records on a KeyField)
     DIA<T>::Sum / Min / Max / AllReduce    thrill/api/sum.hpp, min.hpp, max.hpp, all_reduce.hpp
     DIA<T>::HyperLogLog<p>                 thrill/api/hyperloglog.hpp:62-72 (the registers, not the estimate)
     DIA<T>::Window(k, f[, partial_f])      thrill/api/window.hpp:284-380, :524-564 (the left fold of each window)
@@ -60,6 +60,16 @@ JoinKeyValues = _Functor("(l, r) -> tuple(l.first, l.second, r.second)", capi.JO
 JoinValues = _Functor("(l, r) -> pair(l.second, r.second)", capi.JOIN_VALUES)
 KEY_V1_V2 = np.dtype([("key", "<u8"), ("v1", "<u8"), ("v2", "<u8")])     # std::tuple<uint64_t, V1, V2>, member-wise
 V1_V2 = np.dtype([("v1", "<u8"), ("v2", "<u8")])                         # std::pair<V1, V2>
+# the join function of InnerJoin on records: (l, r) -> std::pair<L, R>, the left item's bytes then the right item's
+JoinPair = _Functor("(l, r) -> pair(l, r)")
+
+
+def KeyField(offset, nbytes):
+    """thrill_gpu::KeyField: the key extractor of InnerJoin on records, the unsigned little-endian integer of nbytes (1..8) bytes at
+    byte offset `offset` of an item, zero-extended to uint64_t"""
+    f = _Functor("KeyField<%d, %d>" % (offset, nbytes))
+    f.key_offset, f.key_bytes = int(offset), int(nbytes)
+    return f
 
 
 def ScanSecond(value_function):
@@ -197,9 +207,14 @@ def Merge(compare_function, *dias, **kw):
 
 
 def InnerJoin(first, second, key_extractor1, key_extractor2, join_function, **kw):
-    """api::InnerJoin(left, right, key_extractor1, key_extractor2, join_function) (api/inner_join.hpp:700-827) on two DIAs of
-    pair<uint64_t, 8-byte value> joined on .first: JoinKeyValues gives KEY_V1_V2 items, JoinValues V1_V2 items.  Worker
-    Hash128to64(0, key) % p holds a key's results, ordered by (key, left global position, right global position)."""
+    """api::InnerJoin(left, right, key_extractor1, key_extractor2, join_function) (api/inner_join.hpp:700-827), in two forms:
+    on two DIAs of pair<uint64_t, 8-byte value> joined on .first (KeyIsFirst), JoinKeyValues gives KEY_V1_V2 items, JoinValues
+    V1_V2 items; on two DIAs of fixed-size records (np.void or structured items, 4..1024 bytes in multiples of 4) joined on a
+    KeyField(offset, nbytes) of each side (KeyIsFirst for pair items), JoinPair gives np.void items of left_bytes + right_bytes,
+    the left item's bytes then the right item's.  Worker Hash128to64(0, key) % p holds a key's results, ordered by (key, left
+    global position, right global position)."""
+    if join_function is JoinPair:
+        return _inner_join_records(first, second, key_extractor1, key_extractor2, kw.get("_pinned_out"))
     if key_extractor1 is not KeyIsFirst or key_extractor2 is not KeyIsFirst:
         raise capi.ThrillGpuError("InnerJoin: only the pair.first key extractors are recognised by the GPU path")
     if join_function not in (JoinKeyValues, JoinValues):
@@ -222,6 +237,44 @@ def InnerJoin(first, second, key_extractor1, key_extractor2, join_function, **kw
     tg.ck(tg.L.tg_inner_join_file(tg.h, C.byref(desc), C.byref(sides[0]), C.byref(sides[1]), C.byref(n_out)))
     dtype = KEY_V1_V2 if join_function is JoinKeyValues else V1_V2
     return DIA(first.ctx, first._fetch(n_out.value, dtype, dtype.itemsize, kw.get("_pinned_out")))
+
+
+def _record_bytes(items):
+    """item size of a DIA of records: np.void or structured items, or rows of a 2-D uint8 array"""
+    if items.ndim == 1 and items.dtype.kind == "V":
+        return items.dtype.itemsize
+    if items.ndim == 2 and items.dtype == np.uint8:
+        return items.shape[1]
+    raise capi.ThrillGpuError("InnerJoin: JoinPair takes DIAs of np.void or structured items, not %r/%r" % (items.dtype, items.shape))
+
+
+def _inner_join_records(first, second, key1, key2, pinned_out):
+    """InnerJoin(left, right, KeyField | KeyIsFirst, KeyField | KeyIsFirst, JoinPair) on DIAs of fixed-size records: np.void
+    items of left_bytes + right_bytes (tg_inner_join_records_file)"""
+    keys = []
+    for k in (key1, key2):
+        if k is KeyIsFirst:
+            keys.append((0, 8))                      # pair<uint64_t, V>: .first is the first 8 bytes
+        elif getattr(k, "key_bytes", None) is not None:
+            keys.append((k.key_offset, k.key_bytes))
+        else:
+            raise capi.ThrillGpuError("InnerJoin: JoinPair takes KeyField or pair.first key extractors, not %r" % (k,))
+    if first.ctx is not second.ctx:
+        raise capi.ThrillGpuError("InnerJoin: the DIAs belong to different contexts")
+    lb, rb = _record_bytes(first.items), _record_bytes(second.items)
+    desc = capi.JoinRecordsDesc(lb, rb, keys[0][0], keys[0][1], keys[1][0], keys[1][1])
+    sides = (capi.MergeInput * 2)()
+    keep = []
+    for j, d in enumerate((first, second)):
+        blocks, nb = d._blocks(d.items)
+        keep.append(blocks)
+        sides[j].blocks = C.cast(blocks, C.POINTER(capi.Block))
+        sides[j].nblocks = nb
+    n_out = C.c_size_t()
+    tg = first.ctx.tg
+    tg.ck(tg.L.tg_inner_join_records_file(tg.h, C.byref(desc), C.byref(sides[0]), C.byref(sides[1]), C.byref(n_out)))
+    dtype = np.dtype((np.void, lb + rb))
+    return DIA(first.ctx, first._fetch(n_out.value, dtype, lb + rb, pinned_out))
 
 
 class GroupIterator(object):

@@ -45,6 +45,11 @@ class JoinDesc(C.Structure):
     _fields_ = [("item_bytes", C.c_uint32), ("join_fn", C.c_uint32)]
 
 
+class JoinRecordsDesc(C.Structure):
+    _fields_ = [("left_bytes", C.c_uint32), ("right_bytes", C.c_uint32), ("left_key_offset", C.c_uint32),
+                ("left_key_bytes", C.c_uint32), ("right_key_offset", C.c_uint32), ("right_key_bytes", C.c_uint32)]
+
+
 class ScanDesc(C.Structure):
     _fields_ = [("item_bytes", C.c_uint32), ("op", C.c_uint32)]
 
@@ -128,6 +133,9 @@ SYMBOLS = [
     ("tg_merge_plan", _i, [_u32, _u32, _P(_u64), _P(_u64), _P(_u64), _P(_u64)]),
     ("tg_inner_join", _i, [_vp, _P(JoinDesc), _vp, _sz, _vp, _sz, _P(_vp), _P(_sz)]),
     ("tg_inner_join_file", _i, [_vp, _P(JoinDesc), _P(MergeInput), _P(MergeInput), _P(_sz)]),
+    ("tg_inner_join_records", _i, [_vp, _P(JoinRecordsDesc), _vp, _sz, _vp, _sz, _P(_vp), _P(_sz)]),
+    ("tg_inner_join_records_file", _i, [_vp, _P(JoinRecordsDesc), _P(MergeInput), _P(MergeInput), _P(_sz)]),
+    ("tg_exchange_records_select", _i, [_vp, _u32, _u32, _u32, _u32, _P(_vp), _P(_sz), _u32, _P(_vp), _P(_sz), _P(_u64)]),
     ("tg_group_by_key", _i, [_vp, _vp, _sz, _P(_vp), _P(_sz)]),
     ("tg_group_to_index", _i, [_vp, _vp, _sz, _u64, _P(_vp), _P(_sz), _P(_u64), _P(_u64)]),
     ("tg_group_by_key_file", _i, [_vp, _P(MergeInput), _P(_sz)]),

@@ -15,7 +15,7 @@
 typedef unsigned long long u64;
 typedef unsigned int u32;
 
-#define TG_NUM_WS 33
+#define TG_NUM_WS 36
 #define TG_MAX_RANKS 16
 
 struct tg_ctx {
@@ -79,7 +79,10 @@ enum { WS_SORT_TMP = 0, WS_SORT_STATUS = 1, WS_SORT_HIST = 2, WS_XCHG_SEND = 3, 
        // Window (tg_window.cu): the all-gathered records and the halo; the output
        WS_WIN_AUX = 28, WS_WIN_OUT = 29,
        // Sample / BernoulliSample (tg_sample.cu): histogram, selection state, records and tile counts; the candidate keys; the output
-       WS_SAMPLE_AUX = 30, WS_SAMPLE_CAND = 31, WS_SAMPLE_OUT = 32 };
+       WS_SAMPLE_AUX = 30, WS_SAMPLE_CAND = 31, WS_SAMPLE_OUT = 32,
+       // InnerJoin on records (tg_join.cu): p > 1, the left side's received records, out of the exchange window's way; an input
+       // that lies in a slot the join writes (an un-detached join or GroupByKey result), copied out of the way (left, right)
+       WS_JOIN_LREC = 33, WS_JOIN_IN_L = 34, WS_JOIN_IN_R = 35 };
 
 int tg_set_error(tg_ctx* ctx, int status, const char* fmt, ...);
 int tg_ws_get(tg_ctx* ctx, int slot, size_t bytes, void** out);

@@ -22,6 +22,7 @@
 #include "tg_keys.cuh"
 #include "tg_segmented.cuh"
 #include "tg_exchange.cuh"
+#include "tg_records.cuh"
 
 using namespace tgp;
 
@@ -543,43 +544,10 @@ int sort_select_impl(tg_ctx* ctx, const tg_key_desc* desc, const KeyView& kv, co
 // Records are a multiple of 4 bytes long and 4-byte aligned: every access below is a 32-bit word, consecutive threads on
 // consecutive words.
 
-// tuple i = { key bytes of record i, i }: one thread per record, the key read as the (<= 4) aligned words that cover it
-__global__ void make_tuples_kernel(const u32* __restrict__ rec, u32 n, u32 rec_words, u32 key_off, u32 key_bytes,
-                                   ulonglong2* __restrict__ tuples) {
-    const u32 stride = gridDim.x * blockDim.x;
-    const u32 w0 = key_off >> 2, sh = 8 * (key_off & 3), nw = (sh ? 1 : 0) + (key_bytes + 3) / 4;
-    for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-        const u32* r = rec + (size_t)i * rec_words + w0;
-        u32 x[5] = { 0, 0, 0, 0, 0 };
-#pragma unroll
-        for (u32 j = 0; j < 4; ++j)
-            if (j < nw && w0 + j < rec_words) x[j] = r[j];
-        u32 k[3];
-#pragma unroll
-        for (u32 j = 0; j < 3; ++j) k[j] = sh ? __funnelshift_r(x[j], x[j + 1], sh) : x[j];
-        // zero the bytes beyond the key
-        if (key_bytes < 12) {
-            const u32 full = key_bytes >> 2, rem = key_bytes & 3;
-#pragma unroll
-            for (u32 j = 0; j < 3; ++j) {
-                if (j > full || (j == full && rem == 0)) k[j] = 0;
-                else if (j == full) k[j] &= (1u << (8 * rem)) - 1;
-            }
-        }
-        tuples[i] = make_ulonglong2(((u64)k[1] << 32) | k[0], ((u64)i << 32) | k[2]);
-    }
-}
-
 // out record j = rec[tuples[j].position]: a CTA moves REC_BATCH consecutive output records per step, thread t the words
 // t, t + 256, ... of the batch (coalesced stores; the words of a record are read by consecutive threads).  Word index lt ->
 // (record, word) by a multiply-high with inv = gather_reciprocal(rec_words), or by a division (DIV) where that is 0.
 constexpr u32 REC_BATCH = 1024;
-// inv = floor((2^32 - 1) / d) + 1 = (2^32 + e) / d with 0 <= e < d, so __umulhi(lt, inv) == lt / d whenever lt * (d - 1) < 2^32:
-// for every word index of a batch (lt < REC_BATCH * d) that holds up to d = 2048.  d = 1 would need inv = 2^32, which does
-// not fit: 4-byte records, and records of more than 8 KiB, take the division.
-inline u32 gather_reciprocal(u32 rec_words) {
-    return rec_words >= 2 && rec_words <= 2048 ? 0xffffffffu / rec_words + 1 : 0u;
-}
 template <bool DIV>
 __global__ void __launch_bounds__(256) gather_records_kernel(const u32* __restrict__ rec, const ulonglong2* __restrict__ tuples,
                                                               u32 n, u32 rec_words, u32 inv, u32* __restrict__ out) {
@@ -656,41 +624,6 @@ int sort_records_local(tg_ctx* ctx, const tg_key_desc* desc, const tg_key_desc& 
     return TG_OK;
 }
 
-// Store step of the records' exchange for worker `me` of p: d_ptup = its n tuples partitioned by destination, counts = the p x p
-// count matrix (host), windows[d] = worker d's window.  Mode 1 stores the records straight into the windows, mode 0 into the
-// local send buffer (WS_XCHG_SEND) followed by the transfers (xchg_transfer).
-int exchange_store_records(tg_ctx* ctx, int mode, bool simulated, const void* d_in, u32 rb, const ulonglong2* d_ptup, size_t n,
-                           const u32* counts, int p, int me, void* const* windows) {
-    u64 before[TG_MAX_RANKS], send_cnt[TG_MAX_RANKS], rc[TG_MAX_RANKS], nr, worst;
-    tg_exchange_plan((u32)p, (u32)me, counts, (uint64_t*)send_cnt, (uint64_t*)rc, (uint64_t*)before, (uint64_t*)&nr, (uint64_t*)&worst);
-    u64 first[TG_MAX_RANKS + 1];                 // first tuple of every destination in the partitioned tuple array
-    first[0] = 0;
-    for (int d = 0; d < TG_MAX_RANKS; ++d) first[d + 1] = first[d] + (d < p ? send_cnt[d] : 0);
-    const int xprof = ctx->profile ? tg_prof_begin(ctx, TG_K_EXCHANGE) : -1;
-    if (mode == 1) {
-        // one launch per destination, every worker starting with its right-hand neighbour: at any time each window is written by
-        // one peer (all workers going through the destinations in the same order would queue up on one NVLink ingress after the other)
-        for (int k = 0; k < p; ++k) {
-            const int d = (me + 1 + k) % p;
-            u32* dst = (u32*)((char*)windows[d] + before[d] * rb);
-            if (send_cnt[d])
-                TG_LAUNCH(ctx, scatter_records_kernel, ctx->sm_count * 8, 256, 0, (const u32*)d_in, d_ptup + first[d],
-                          (u32)send_cnt[d], rb / 4, 0u, dst);
-        }
-    }
-    else {
-        char* d_send;
-        TG_TRY(tg_ws_get(ctx, WS_XCHG_SEND, (n + 1) * (size_t)rb, (void**)&d_send));
-        for (int d = 0; d < p; ++d)
-            if (send_cnt[d])
-                TG_LAUNCH(ctx, scatter_records_kernel, ctx->sm_count * 8, 256, 0, (const u32*)d_in, d_ptup + first[d],
-                          (u32)send_cnt[d], rb / 4, 0u, (u32*)(d_send + (size_t)first[d] * rb));
-        TG_TRY(xchg_transfer(ctx, simulated, d_send, rb, counts, p, me, windows));
-    }
-    if (xprof >= 0) tg_prof_end(ctx, xprof);
-    return TG_OK;
-}
-
 int sort_records_impl(tg_ctx* ctx, const tg_key_desc* desc, void* d_in, size_t n_local, uint64_t rng_seed,
                       void** out_dptr, size_t* out_n) {
     const u32 rb = desc->item_bytes;
@@ -742,25 +675,6 @@ int sort_records_impl(tg_ctx* ctx, const tg_key_desc* desc, void* d_in, size_t n
 
 // ---- tg_exchange_select: one exchange for p simulated workers, one after another on the ctx's stream ----------------------------
 // (never two workers' passes at once: the look-back of the partition pass sizes its grid assuming every CTA is resident)
-
-// after the count steps: out_counts, the receive limit and the windows' sizes, before any store
-int select_check(tg_ctx* ctx, const u32* h_mat, int p, size_t s, void* const* d_windows, const size_t* window_bytes, uint64_t* out_counts) {
-    for (int i = 0; i < p * p; ++i) out_counts[i] = h_mat[i];
-    u64 sc[TG_MAX_RANKS], rc[TG_MAX_RANKS], before[TG_MAX_RANKS], nr, worst;
-    tg_exchange_plan((u32)p, 0, h_mat, (uint64_t*)sc, (uint64_t*)rc, (uint64_t*)before, (uint64_t*)&nr, (uint64_t*)&worst);
-    if (worst >= (1u << 30))
-        return tg_set_error(ctx, TG_ERR_TOO_LARGE, "exchange_select: a worker would receive %llu items (limit 2^30 - 1)", (unsigned long long)worst);
-    if (!d_windows) return TG_OK;
-    if (!window_bytes) return tg_set_error(ctx, TG_ERR_ARG, "exchange_select: windows without their sizes");
-    for (int d = 0; d < p; ++d) {
-        u64 recv = 0;
-        for (int src = 0; src < p; ++src) recv += h_mat[src * p + d];
-        if ((recv && !d_windows[d]) || window_bytes[d] < recv * s)
-            return tg_set_error(ctx, TG_ERR_ARG, "exchange_select: window %d holds %zu bytes, receives %llu", d, window_bytes[d],
-                                (unsigned long long)(recv * s));
-    }
-    return TG_OK;
-}
 
 // 8- or 16-byte items by fn; prep(w) sets up worker w's state of fn (the splitters) before each of its steps
 template <int WORDS, class DigitFn, class Prep>
@@ -833,6 +747,64 @@ int select_records(tg_ctx* ctx, int mode, const tg_key_desc* desc, uint64_t rng_
 }
 
 }  // namespace
+
+namespace tgp {
+
+// Store step of the records' exchange for worker `me` of p: d_ptup = its n tuples partitioned by destination, counts = the p x p
+// count matrix (host), windows[d] = worker d's window.  Mode 1 stores the records straight into the windows, mode 0 into the
+// local send buffer (WS_XCHG_SEND) followed by the transfers (xchg_transfer).
+int exchange_store_records(tg_ctx* ctx, int mode, bool simulated, const void* d_in, u32 rb, const ulonglong2* d_ptup, size_t n,
+                           const u32* counts, int p, int me, void* const* windows) {
+    u64 before[TG_MAX_RANKS], send_cnt[TG_MAX_RANKS], rc[TG_MAX_RANKS], nr, worst;
+    tg_exchange_plan((u32)p, (u32)me, counts, (uint64_t*)send_cnt, (uint64_t*)rc, (uint64_t*)before, (uint64_t*)&nr, (uint64_t*)&worst);
+    u64 first[TG_MAX_RANKS + 1];                 // first tuple of every destination in the partitioned tuple array
+    first[0] = 0;
+    for (int d = 0; d < TG_MAX_RANKS; ++d) first[d + 1] = first[d] + (d < p ? send_cnt[d] : 0);
+    const int xprof = ctx->profile ? tg_prof_begin(ctx, TG_K_EXCHANGE) : -1;
+    if (mode == 1) {
+        // one launch per destination, every worker starting with its right-hand neighbour: at any time each window is written by
+        // one peer (all workers going through the destinations in the same order would queue up on one NVLink ingress after the other)
+        for (int k = 0; k < p; ++k) {
+            const int d = (me + 1 + k) % p;
+            u32* dst = (u32*)((char*)windows[d] + before[d] * rb);
+            if (send_cnt[d])
+                TG_LAUNCH(ctx, scatter_records_kernel, ctx->sm_count * 8, 256, 0, (const u32*)d_in, d_ptup + first[d],
+                          (u32)send_cnt[d], rb / 4, 0u, dst);
+        }
+    }
+    else {
+        char* d_send;
+        TG_TRY(tg_ws_get(ctx, WS_XCHG_SEND, (n + 1) * (size_t)rb, (void**)&d_send));
+        for (int d = 0; d < p; ++d)
+            if (send_cnt[d])
+                TG_LAUNCH(ctx, scatter_records_kernel, ctx->sm_count * 8, 256, 0, (const u32*)d_in, d_ptup + first[d],
+                          (u32)send_cnt[d], rb / 4, 0u, (u32*)(d_send + (size_t)first[d] * rb));
+        TG_TRY(xchg_transfer(ctx, simulated, d_send, rb, counts, p, me, windows));
+    }
+    if (xprof >= 0) tg_prof_end(ctx, xprof);
+    return TG_OK;
+}
+
+// after the count steps: out_counts, the receive limit and the windows' sizes, before any store
+int select_check(tg_ctx* ctx, const u32* h_mat, int p, size_t s, void* const* d_windows, const size_t* window_bytes, uint64_t* out_counts) {
+    for (int i = 0; i < p * p; ++i) out_counts[i] = h_mat[i];
+    u64 sc[TG_MAX_RANKS], rc[TG_MAX_RANKS], before[TG_MAX_RANKS], nr, worst;
+    tg_exchange_plan((u32)p, 0, h_mat, (uint64_t*)sc, (uint64_t*)rc, (uint64_t*)before, (uint64_t*)&nr, (uint64_t*)&worst);
+    if (worst >= (1u << 30))
+        return tg_set_error(ctx, TG_ERR_TOO_LARGE, "exchange_select: a worker would receive %llu items (limit 2^30 - 1)", (unsigned long long)worst);
+    if (!d_windows) return TG_OK;
+    if (!window_bytes) return tg_set_error(ctx, TG_ERR_ARG, "exchange_select: windows without their sizes");
+    for (int d = 0; d < p; ++d) {
+        u64 recv = 0;
+        for (int src = 0; src < p; ++src) recv += h_mat[src * p + d];
+        if ((recv && !d_windows[d]) || window_bytes[d] < recv * s)
+            return tg_set_error(ctx, TG_ERR_ARG, "exchange_select: window %d holds %zu bytes, receives %llu", d, window_bytes[d],
+                                (unsigned long long)(recv * s));
+    }
+    return TG_OK;
+}
+
+}  // namespace tgp
 
 extern "C" {
 

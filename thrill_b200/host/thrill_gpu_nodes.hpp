@@ -7,6 +7,7 @@
  *     thrill_gpu::ReducePair(dia, std::plus<double> ...)          <->  DIA<T>::ReducePair(api/reduce_by_key.hpp:410)
  *     thrill_gpu::Merge(std::less<T>(), dia0, dia1, ...)          <->  api::Merge        (api/merge.hpp:673)
  *     thrill_gpu::InnerJoin(l, r, KeyFirst(), KeyFirst(), JoinValues()) <->  api::InnerJoin (api/inner_join.hpp:700)
+ *     thrill_gpu::InnerJoin(l, r, KeyField<L>(), KeyField<R>(), JoinPair<L, R>()) <->  api::InnerJoin on records
  *     thrill_gpu::GroupByKey<Out>(dia, KeyFirst(), fn)            <->  DIA<T>::GroupByKey (api/group_by_key.hpp:419)
  *     thrill_gpu::GroupToIndex<Out>(dia, KeyFirst(), fn, size)    <->  DIA<T>::GroupToIndex (api/group_to_index.hpp:257)
  *     thrill_gpu::PrefixSum(dia, fn [, initial]) / ExPrefixSum    <->  DIA<T>::PrefixSum / ExPrefixSum (api/dia.hpp:1850, :1867)
@@ -235,6 +236,44 @@ template <>
 struct JoinDesc<JoinValues>{
     static constexpr bool supported = true;
     static constexpr uint32_t fn = TG_JOIN_VALUES, out_bytes = 16;
+};
+
+//! InnerJoin on records: DIAs of trivially copyable PODs (serialized as their raw sizeof(T) bytes, data/serialization.hpp) joined
+//! on an unsigned little-endian integer field of 1..8 bytes at any byte offset.  Name an item type's key field by specialising
+//!   template <> struct thrill_gpu::UintKeyTraits<LineItem> { static constexpr bool is_uint_key = true;
+//!                                                            static constexpr uint32_t key_offset = 0, key_bytes = 8; };
+//! KeyField<T> extracts it (zero-extended to uint64_t) and JoinPair<L, R> makes std::pair<L, R> of the two items.  Both are
+//! plain functors with one operator(), so the stock api::InnerJoin takes the same call.
+template <typename ValueType>
+struct UintKeyTraits {
+    static constexpr bool is_uint_key = false;
+};
+template <typename T>
+struct KeyField {
+    uint64_t operator () (const T& item) const {
+        static_assert(UintKeyTraits<T>::is_uint_key, "thrill_gpu::KeyField<T>: specialise thrill_gpu::UintKeyTraits<T>");
+        uint64_t key = 0;
+        std::memcpy(&key, reinterpret_cast<const char*>(&item) + UintKeyTraits<T>::key_offset, UintKeyTraits<T>::key_bytes);
+        return key;
+    }
+};
+template <typename L, typename R>
+struct JoinPair {
+    std::pair<L, R> operator () (const L& l, const R& r) const { return std::make_pair(l, r); }
+};
+//! the record layout of an item type with a key extractor: a POD with KeyField<T> (sizeof(T) bytes), or pair<uint64_t, V>
+//! with KeyFirst (8 + sizeof(V) bytes, serialized member-wise, the key first)
+template <typename T, typename KeyExtractor>
+struct RecordKey { static constexpr bool supported = false; };
+template <typename T>
+struct RecordKey<T, KeyField<T> >{
+    static constexpr bool supported = UintKeyTraits<T>::is_uint_key && std::is_pod<T>::value;
+    static constexpr uint32_t bytes = sizeof(T), key_offset = UintKeyTraits<T>::key_offset, key_bytes = UintKeyTraits<T>::key_bytes;
+};
+template <typename V>
+struct RecordKey<std::pair<uint64_t, V>, KeyFirst>{
+    static constexpr bool supported = std::is_pod<V>::value;
+    static constexpr uint32_t bytes = 8 + sizeof(V), key_offset = 0, key_bytes = 8;
 };
 
 //! The sum function thrill_gpu::PrefixSum / ExPrefixSum recognise on pair<uint64_t, V>: F (one of the ReducePair functions,
@@ -718,9 +757,18 @@ private:
 
 //! api::InnerJoin (api/inner_join.hpp:700-827): the JoinNode protocol (one File per parent, registered with
 //! AddChild(this, chain, index), :133-157; StopPreOp per parent) with the hash exchange, the local sorts and the join of
-//! Execute / PushData (:159-312) behind tg_inner_join_file.  Either side may arrive as a device File from a parent GPU node.
-//! kOutBytes: the serialized size of ValueType (24 for the (key, v1, v2) tuple, 16 for the (v1, v2) pair).
-template <typename ValueType, typename LeftType, typename RightType, uint32_t kOutBytes>
+//! Execute / PushData (:159-312) behind tg_inner_join_file (pairs, Desc = tg_join_desc) or tg_inner_join_records_file (records,
+//! Desc = tg_join_records_desc).  Either side may arrive as a device File from a parent GPU node.  kOutBytes: the serialized size
+//! of ValueType (24 for the (key, v1, v2) tuple, 16 for the (v1, v2) pair, left_bytes + right_bytes for JoinPair).
+inline uint32_t JoinInputBytes(const tg_join_desc& d, size_t) { return d.item_bytes; }
+inline uint32_t JoinInputBytes(const tg_join_records_desc& d, size_t i) { return i ? d.right_bytes : d.left_bytes; }
+inline void JoinFile(tg_ctx* c, const tg_join_desc& d, const tg_merge_input* l, const tg_merge_input* r, size_t* n) {
+    Check(c, tg_inner_join_file(c, &d, l, r, n), "tg_inner_join_file");
+}
+inline void JoinFile(tg_ctx* c, const tg_join_records_desc& d, const tg_merge_input* l, const tg_merge_input* r, size_t* n) {
+    Check(c, tg_inner_join_records_file(c, &d, l, r, n), "tg_inner_join_records_file");
+}
+template <typename ValueType, typename LeftType, typename RightType, uint32_t kOutBytes, typename Desc = tg_join_desc>
 class GpuJoinNode final : public thrill::api::DOpNode<ValueType>, public GpuNodeBase
 {
     using Super = thrill::api::DOpNode<ValueType>;
@@ -728,7 +776,7 @@ class GpuJoinNode final : public thrill::api::DOpNode<ValueType>, public GpuNode
 
 public:
     template <typename LeftDIA, typename RightDIA>
-    GpuJoinNode(const LeftDIA& left, const RightDIA& right, const tg_join_desc& desc)
+    GpuJoinNode(const LeftDIA& left, const RightDIA& right, const Desc& desc)
         : Super(left.ctx(), "GpuInnerJoin", { left.id(), right.id() }, { left.node(), right.node() }),
           desc_(desc), parent_stack_empty_({ { LeftDIA::stack_empty, RightDIA::stack_empty } }) {
         for (size_t i = 0; i < 2; ++i) {
@@ -750,7 +798,7 @@ public:
     }
 
     bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes, size_t parent_index) final {
-        if (!parent_stack_empty_[parent_index] || item_bytes != 16) return false;
+        if (!parent_stack_empty_[parent_index] || item_bytes != JoinInputBytes(desc_, parent_index)) return false;
         device_inputs_[parent_index] = file;
         return true;
     }
@@ -759,7 +807,7 @@ public:
 
     DIAMemUse ExecuteMemUse() final { return DIAMemUse::Max(); }
 
-    //! both exchanges, the local sorts and the join behind tg_inner_join_file.  Collective.  The result stays in HBM.
+    //! both exchanges, the local sorts and the join behind tg_inner_join(_records)_file.  Collective.  The result stays in HBM.
     void Execute() final {
         tg_ctx* c = WorkerCtx(context_);
         std::vector<std::unique_ptr<PinnedFileView> > views;
@@ -773,7 +821,7 @@ public:
             in[i] = tg_merge_input { nullptr, views.back()->data(), views.back()->size() };
         }
         size_t out_items = 0;
-        Check(c, tg_inner_join_file(c, &desc_, &in[0], &in[1], &out_items), "tg_inner_join_file");
+        JoinFile(c, desc_, &in[0], &in[1], &out_items);
         views.clear();
         for (size_t i = 0; i < 2; ++i) {
             files_[i]->Clear();
@@ -806,7 +854,7 @@ public:
     void Dispose() final { joined_file_.Clear(); device_result_.reset(); have_host_file_ = false; }
 
 private:
-    tg_join_desc desc_;
+    Desc desc_;
     const std::array<bool, 2> parent_stack_empty_;
     thrill::data::FilePtr files_[2];
     thrill::data::File::Writer writers_[2];
@@ -1476,12 +1524,19 @@ auto Merge(const Comparator& /* comparator */, const FirstDIA& first_dia, const 
     return DIA<ValueType>(node);
 }
 
+//! JoinPair calls take the records' front door below
+template <typename JoinFunction>
+struct IsJoinPair : std::false_type { };
+template <typename L, typename R>
+struct IsJoinPair<JoinPair<L, R> >: std::true_type { };
+
 //! api::InnerJoin(left, right, key_extractor1, key_extractor2, join_function) (api/inner_join.hpp:700-827) for pair DIAs joined on
 //! .first: left = DIA<pair<uint64_t, V1>>, right = DIA<pair<uint64_t, V2>> with 8-byte V1 and V2, key extractors KeyFirst,
 //! join_function JoinKeyValues (-> tuple<uint64_t, V1, V2>) or JoinValues (-> pair<V1, V2>).  Worker Hash128to64(0, key) % p
 //! holds a key's results, ordered by (key, left global position, right global position), one of the orders the stock operator
 //! allows.  InnerJoin(a, a, ...) is a self-join with one parent on both edges.
-template <typename LeftDIA, typename RightDIA, typename JoinFunction>
+template <typename LeftDIA, typename RightDIA, typename JoinFunction,
+          typename = typename std::enable_if<!IsJoinPair<JoinFunction>::value>::type>
 auto InnerJoin(const LeftDIA& left, const RightDIA& right, const KeyFirst& /* key_extractor1 */,
                const KeyFirst& /* key_extractor2 */, const JoinFunction& join_function) {
     using LeftType = typename LeftDIA::ValueType;
@@ -1501,6 +1556,38 @@ auto InnerJoin(const LeftDIA& left, const RightDIA& right, const KeyFirst& /* ke
     right.AssertValid();
     auto node = tlx::make_counting<GpuJoinNode<ValueType, LeftType, RightType, JoinDesc<JoinFunction>::out_bytes> >(
         left, right, tg_join_desc { 16, JoinDesc<JoinFunction>::fn });
+    return DIA<ValueType>(node);
+}
+
+//! api::InnerJoin on records (api/inner_join.hpp:700-827): left = DIA<L>, right = DIA<R>, each a POD whose key field is named by
+//! UintKeyTraits (key extractor KeyField<T>) or a pair<uint64_t, V> with a POD V (key extractor KeyFirst), serialized sizes a
+//! multiple of 4 from 4 to 1024 bytes; join_function JoinPair<L, R> (-> std::pair<L, R>, the left item's bytes then the right
+//! item's).  Keys are compared as zero-extended uint64_t.  Worker Hash128to64(0, key) % p holds a key's results, ordered by (key,
+//! left global position, right global position), one of the orders the stock operator allows.  InnerJoin(a, a, ...) is a
+//! self-join with one parent on both edges.  Packed structs whose size is not a multiple of 4, other join functions, signed keys
+//! or keys of more than 8 bytes, location detection and outer joins are not built: use the stock api::InnerJoin.
+template <typename LeftDIA, typename RightDIA, typename KeyExtractor1, typename KeyExtractor2, typename L, typename R>
+auto InnerJoin(const LeftDIA& left, const RightDIA& right, const KeyExtractor1& /* key_extractor1 */,
+               const KeyExtractor2& /* key_extractor2 */, const JoinPair<L, R>& /* join_function */) {
+    using LK = RecordKey<typename LeftDIA::ValueType, KeyExtractor1>;
+    using RK = RecordKey<typename RightDIA::ValueType, KeyExtractor2>;
+    static_assert(std::is_same<typename LeftDIA::ValueType, L>::value && std::is_same<typename RightDIA::ValueType, R>::value,
+                  "thrill_gpu::InnerJoin: JoinPair<L, R> must name the two DIAs' item types");
+    static_assert(LK::supported && RK::supported,
+                  "thrill_gpu::InnerJoin: records need a POD with KeyField<T> (UintKeyTraits) or pair<uint64_t, POD> with KeyFirst; "
+                  "use the stock api::InnerJoin(left, right, key1, key2, join_fn)");
+    static_assert(LK::bytes % 4 == 0 && LK::bytes <= 1024 && RK::bytes % 4 == 0 && RK::bytes <= 1024,
+                  "thrill_gpu::InnerJoin: record sizes must be multiples of 4 bytes, at most 1024 (packed structs of other sizes: "
+                  "use the stock api::InnerJoin(left, right, key1, key2, join_fn))");
+    static_assert(LK::key_bytes >= 1 && LK::key_bytes <= 8 && LK::key_offset + LK::key_bytes <= LK::bytes &&
+                  RK::key_bytes >= 1 && RK::key_bytes <= 8 && RK::key_offset + RK::key_bytes <= RK::bytes,
+                  "thrill_gpu::InnerJoin: keys are unsigned integers of 1..8 bytes inside the item (longer or signed keys: use the "
+                  "stock api::InnerJoin(left, right, key1, key2, join_fn))");
+    using ValueType = std::pair<L, R>;
+    left.AssertValid();
+    right.AssertValid();
+    auto node = tlx::make_counting<GpuJoinNode<ValueType, L, R, LK::bytes + RK::bytes, tg_join_records_desc> >(
+        left, right, tg_join_records_desc { LK::bytes, RK::bytes, LK::key_offset, LK::key_bytes, RK::key_offset, RK::key_bytes });
     return DIA<ValueType>(node);
 }
 
