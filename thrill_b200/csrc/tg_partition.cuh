@@ -117,6 +117,13 @@ struct PartCfg {
 // the members before it with the first batch of its look-back (G <= LB in partition_kernel).
 constexpr u32 TILE_GROUP = 8;
 
+// What the write-out of a pass does besides storing each item at its position: nothing (NoFinish), or, in the radix sort's
+// last prefix pass, ordering the groups of equal key prefix that lie inside the exchange buffer (FusedFinish,
+// tg_radix_sort.cu).  kOn selects the write-out at compile time: the passes without it compile as before.
+struct NoFinish {
+    static constexpr bool kOn = false;
+};
+
 // exclusive scan of npass digit histograms -> global bases; skip[p] = 1 if one bin holds everything
 static __global__ void scan_hist_kernel(const u32* __restrict__ ghist, u32* __restrict__ gbase, u32* __restrict__ skip,
                                  int npass, u32 n) {
@@ -219,11 +226,12 @@ __device__ __forceinline__ u32 seg_num_tiles(const SegList& sl) { return sl.num_
 // PEER: the buckets are destination workers; bucket d is written to dbase[d][position], where dbase[d] points into worker
 // d's exchange window (mapped peer memory: the stores travel over NVLink) biased so that `position` is the position the
 // plain pass would have used in `out` — the Alltoallv of the reference's MixStream exchange happens inside the pass.
-template <int WORDS, class DigitFn, bool SEG, bool PEER, bool UNSTABLE>
+// Fin: the write-out (NoFinish, or the radix sort's fused finishing pass: see FusedFinish in tg_radix_sort.cu).
+template <int WORDS, class DigitFn, bool SEG, bool PEER, bool UNSTABLE, class Fin = NoFinish>
 __global__ void __launch_bounds__(PartCfg<WORDS>::THREADS, PartCfg<WORDS>::MIN_BLOCKS)
 partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename ItemT<WORDS>::type* __restrict__ out,
                  u32 n, const DigitFn fn_param, const u32* __restrict__ gbase, u32* __restrict__ status, const SegList sl,
-                 typename ItemT<WORDS>::type* const* __restrict__ dbase) {
+                 typename ItemT<WORDS>::type* const* __restrict__ dbase, const Fin fin) {
     typedef typename ItemT<WORDS>::type Item;
     typedef PartCfg<WORDS, DigitFn::kStoreDigit, PEER, DigitFn::kScratch> C;
     constexpr int THREADS = C::THREADS, ITEMS = C::ITEMS, TILE = C::TILE, HALF = C::HALF, NWARPS = C::NWARPS;
@@ -234,6 +242,8 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
     constexpr int LB = 8;
     static_assert(TILE_GROUP <= (u32)LB, "a group member reaches past its group's first tile with one batch");
     static_assert(THREADS >= RADIX, "one thread per digit in the scan phases");
+    static_assert(!Fin::kOn || (SEG && !PEER && !UNSTABLE && !DigitFn::kStoreDigit && !DigitFn::kHasDrop),
+                  "the fused finishing pass is a stable segmented pass of the radix sort");
 
     // plain pointer arithmetic on the shared array keeps the shared address space (LDS/STS, 32-bit addresses)
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -475,7 +485,12 @@ partition_kernel(const typename ItemT<WORDS>::type* __restrict__ in, typename It
             __syncthreads();
 
             // ---- coalesced write-out: consecutive threads write consecutive addresses inside a digit run
-            {
+            if constexpr (Fin::kOn) {
+                const u32 q0r = (u32)(r * HALF);
+                const u32 nr = tile_valid > q0r ? (tile_valid - q0r < (u32)HALF ? tile_valid - q0r : (u32)HALF) : 0u;
+                fin.template write_out<THREADS, HALF / THREADS>(xbuf, nr, q0r, goff, fn, out, tid);
+            }
+            else {
                 const Item* const bufp = xbuf + tid;
                 const u32 q0 = (u32)(r * HALF) + tid;        // tile-local position of bufp[0]
                 if (full_tile) {
@@ -519,12 +534,12 @@ constexpr u32 tile_items() { return (u32)PartCfg<WORDS>::TILE; }
 template <int WORDS>
 constexpr u32 num_tiles_for(size_t n) { return (u32)((n + tile_items<WORDS>() - 1) / tile_items<WORDS>()); }
 
-template <int WORDS, class DigitFn, bool SEG, bool PEER = false, bool UNSTABLE = false>
+template <int WORDS, class DigitFn, bool SEG, bool PEER = false, bool UNSTABLE = false, class Fin = NoFinish>
 int launch_partition_v(tg_ctx* ctx, const void* in, void* out, u32 n, const DigitFn& fn, const u32* gbase, u32* status,
-                       const SegList& sl, typename ItemT<WORDS>::type* const* dbase = nullptr) {
+                       const SegList& sl, typename ItemT<WORDS>::type* const* dbase = nullptr, const Fin& fin = Fin()) {
     typedef typename ItemT<WORDS>::type Item;
     typedef PartCfg<WORDS, DigitFn::kStoreDigit, PEER, DigitFn::kScratch> C;
-    auto kern = partition_kernel<WORDS, DigitFn, SEG, PEER, UNSTABLE>;
+    auto kern = partition_kernel<WORDS, DigitFn, SEG, PEER, UNSTABLE, Fin>;
     int ctas_per_sm = 0;
     auto it = ctx->kernel_cfg.find((const void*)kern);
     if (it != ctx->kernel_cfg.end()) ctas_per_sm = it->second;
@@ -540,7 +555,7 @@ int launch_partition_v(tg_ctx* ctx, const void* in, void* out, u32 n, const Digi
     if (num_tiles == 0) return TG_OK;
     int grid = ctx->sm_count * ctas_per_sm;
     if (grid > (int)num_tiles) grid = (int)num_tiles;
-    TG_LAUNCH_T(ctx, TG_K_PARTITION, kern, grid, C::THREADS, C::SMEM, (const Item*)in, (Item*)out, n, fn, gbase, status, sl, dbase);
+    TG_LAUNCH_T(ctx, TG_K_PARTITION, kern, grid, C::THREADS, C::SMEM, (const Item*)in, (Item*)out, n, fn, gbase, status, sl, dbase, fin);
     return TG_OK;
 }
 

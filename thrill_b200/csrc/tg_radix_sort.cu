@@ -5,8 +5,10 @@
 //
 // Prefix sort (the fast path, prefix_sort_fast): one counting read (chunk histograms of the most significant key byte +
 // OR/AND of all keys), the pass on that byte as a chunked pass, the next K-1 non-constant bytes as segmented passes inside
-// its buckets (tg_segmented.cuh), and one finishing pass that orders the short runs of equal K-byte prefixes by the full
-// key (prefix_fixup_kernel); K = ceil((log2 n + 4) / 8).  8 + K*16 + 8 + 16 bytes per 8-byte key.
+// its buckets (tg_segmented.cuh), and the finishing step that orders the short runs of equal K-byte prefixes by the full
+// key: fused into the last of those passes plus a repair of the runs it cannot see whole (FusedFinish,
+// finish_repair_kernel), or a separate pass (prefix_fixup_kernel); K = ceil((log2 n + 4) / 8).  8 + K*16 + 8 bytes per
+// 8-byte key (+ 16 with the separate pass).
 // General path (few non-constant bytes, long runs of equal prefixes, small inputs): one histogram kernel (all digit
 // histograms from a single read), one tiny scan kernel, then one stable partition pass per non-constant 8-bit digit,
 // least significant first (chained scan).  n*s for the histogram + per pass n*s read + n*s write (s = item bytes).
@@ -252,6 +254,200 @@ __global__ void __launch_bounds__(FIX_THREADS) prefix_fixup_kernel(const typenam
     }
 }
 
+// ---- the finishing pass fused into the last prefix pass -----------------------------------------------------------
+// The last pass on a prefix digit holds each tile's items in prefix order in its exchange buffer (the tile lies inside one
+// segment, which the earlier passes ordered by the lower prefix digits): every group of equal prefixes that lies inside an
+// exchange round is a run of neighbours there.  Its write-out orders those runs the way fixup_group_member does (rank =
+// smaller full keys, ties by position: stable), so the separate finishing pass, one more read and write of every item, is
+// not needed.  Groups that cross a piece of a digit run — a boundary between two tiles' runs of the same digit, or the
+// boundary between a tile's two exchange rounds — are ordered piece by piece; finish_repair_kernel then re-sorts them whole.
+template <bool PLAIN>
+struct FusedFinish {
+    static constexpr bool kOn = true;
+    KeyView kv;
+    PrefixMask pm;
+    u32* fail;
+
+    template <class Item>
+    __device__ __forceinline__ Canon full(const Item& v) const { return fix_canon<PLAIN>(v, kv); }
+    // the key's prefix bits (PLAIN: in .lo only)
+    template <class Item>
+    __device__ __forceinline__ Canon prefix(const Item& v) const {
+        const Canon c = full(v);
+        Canon p;
+        p.hi = PLAIN ? 0 : c.hi & pm.hi;
+        p.lo = c.lo & pm.lo;
+        return p;
+    }
+    __device__ __forceinline__ static bool eq(const Canon& a, const Canon& b) { return PLAIN ? a.lo == b.lo : canon_eq(a, b); }
+
+    // an item of a group of more than one in xb[0, nr): its rank in the group -> dst[head + rank]; a group of more than FIX_H
+    // items sets *fail (the same limit as prefix_fixup_kernel; every member finds it) and leaves its members where they are
+    template <class Item>
+    __device__ __forceinline__ void member(const Item* xb, u32 x, u32 nr, Item* dst) const {
+        const Item me = xb[x];
+        const Canon k = full(me), pk = prefix(me);
+        u32 lo = x, hi = x;
+        bool bad = false;
+        while (lo > 0 && eq(prefix(xb[lo - 1]), pk)) {
+            --lo;
+            if (x - lo >= (u32)FIX_H) { bad = true; break; }
+        }
+        while (!bad && hi + 1 < nr && eq(prefix(xb[hi + 1]), pk)) {
+            ++hi;
+            if (hi - lo >= (u32)FIX_H) bad = true;
+        }
+        if (bad) {
+            *fail = 1;
+            dst[x] = me;
+            return;
+        }
+        u32 rank = 0;
+        for (u32 y = lo; y <= hi; ++y) {
+            const Canon c = full(xb[y]);
+            rank += (canon_less(c, k) || (y < x && canon_eq(c, k))) ? 1u : 0u;
+        }
+        dst[lo + rank] = me;
+    }
+
+    // write-out of one exchange round: xb[0, nr) holds tile positions [q0, q0 + nr); item x of digit d goes to
+    // out[goff[d] + q0 + x].  Items whose neighbours have other prefixes (nearly all of them) are stored in the first loop,
+    // as the plain write-out does; the group members are flagged and ordered after it, so that a warp branches once per
+    // member it holds, not once per store.  The positions outside [0, nr) count as other prefixes.
+    template <int THREADS, int IT, class Item, class DigitFn>
+    __device__ __forceinline__ void write_out(const Item* xb, u32 nr, u32 q0, const u32* goff, const DigitFn& fn, Item* out,
+                                              int tid) const {
+        const u32 lane = (u32)tid & 31u;
+        u32 mem = 0;         // bit i: the item at xb[i * THREADS + tid] is a group member
+#pragma unroll
+        for (int i = 0; i < IT; ++i) {
+            const u32 x = (u32)(i * THREADS + tid);
+            const Item v = xb[x];
+            const Canon p = prefix(v);
+            Canon pl, pr;          // the neighbours' prefixes
+            bool has_l = x > 0, has_r = x + 1 < nr;
+            if (PLAIN) {
+                // plain keys: both neighbours from the buffer, no branch (the loads of all iterations can be issued together)
+                pl = prefix(xb[x > 0 ? x - 1 : 0]);
+                pr = prefix(xb[x + 1 < (u32)(IT * THREADS) ? x + 1 : x]);
+            }
+            else {
+                // canonical keys cost more to form: from the neighbouring lanes, lanes 0 and 31 from the buffer
+                pl.lo = __shfl_up_sync(0xffffffffu, p.lo, 1);
+                pr.lo = __shfl_down_sync(0xffffffffu, p.lo, 1);
+                pl.hi = __shfl_up_sync(0xffffffffu, p.hi, 1);
+                pr.hi = __shfl_down_sync(0xffffffffu, p.hi, 1);
+                const u32 y = lane == 0 ? x - 1 : x + 1;      // (x - 1 wraps to >= nr at x = 0)
+                bool edge = false;
+                if ((lane == 0 || lane == 31) && y < nr) {
+                    const Canon e = prefix(xb[y]);
+                    if (lane == 0) pl = e; else pr = e;
+                    edge = true;
+                }
+                if (lane == 0) has_l = edge;
+                if (lane == 31) has_r = edge;
+            }
+            if (x < nr) {
+                if ((has_l && eq(pl, p)) || (has_r && eq(pr, p))) mem |= 1u << i;
+                else out[goff[fn(v, 0)] + q0 + x] = v;
+            }
+        }
+        while (mem) {
+            const int i = __ffs(mem) - 1;
+            mem &= mem - 1;
+            const u32 x = (u32)(i * THREADS + tid);
+            member(xb, x, nr, out + goff[fn(xb[x], 0)] + q0);
+        }
+    }
+
+    // finish_repair_kernel: is p (0 < p < n) inside a group of equal prefixes?  Then the thread that first claims the group's
+    // head re-sorts the whole group in place by (full key, position): stable, since the pieces were ordered stably and lie in
+    // input order.  The other threads that meet the group only read it, and every position of it holds one of its items at
+    // any time, so they find the same head.
+    template <class Item>
+    __device__ __forceinline__ void repair(Item* out, u32 n, u32 p, u32* claim) const {
+        const Canon pk = prefix(out[p]);
+        if (!eq(prefix(out[p - 1]), pk)) return;
+        u32 h = p - 1;
+        while (h > 0 && eq(prefix(out[h - 1]), pk)) {
+            --h;
+            if (p - h >= (u32)FIX_H) { *fail = 1; return; }
+        }
+        const u32 bit = 1u << (h & 31);
+        if (atomicOr(&claim[h >> 5], bit) & bit) return;
+        u32 e = p;
+        while (e + 1 < n && eq(prefix(out[e + 1]), pk)) {
+            ++e;
+            if (e - h >= (u32)FIX_H) { *fail = 1; return; }
+        }
+        const u32 len = e - h + 1;
+        unsigned char rk[FIX_H];
+        for (u32 x = 0; x < len; ++x) {
+            const Canon k = full(out[h + x]);
+            u32 r = 0;
+            for (u32 y = 0; y < len; ++y) {
+                const Canon c = full(out[h + y]);
+                r += (canon_less(c, k) || (y < x && canon_eq(c, k))) ? 1u : 0u;
+            }
+            rk[x] = (unsigned char)r;
+        }
+        u64 placed = 0;      // apply the permutation x -> rk[x] cycle by cycle
+        for (u32 x = 0; x < len; ++x) {
+            if ((placed >> x) & 1u) continue;
+            Item v = out[h + x];
+            u32 y = rk[x];
+            placed |= 1ull << x;
+            while (y != x) {
+                const Item w = out[h + y];
+                out[h + y] = v;
+                v = w;
+                placed |= 1ull << y;
+                y = rk[y];
+            }
+            out[h + x] = v;
+        }
+    }
+};
+
+// After a fused last pass: one CTA per tile of its tile list, one thread per digit.  The boundaries where a group can be cut
+// are the start of every nonempty run of a digit (its position follows from the pass's final inclusive status rows and
+// segbase) and the position of a tile's second exchange round inside the digit run that holds it.  Each is checked once.
+// claim: one zeroed bit per position (a group's head, taken by the one thread that re-sorts it).
+template <int WORDS, bool PLAIN>
+__global__ void __launch_bounds__(RADIX) finish_repair_kernel(typename ItemT<WORDS>::type* out, u32 n, const SegList sl,
+                                                              const u32* __restrict__ status, u32* __restrict__ claim,
+                                                              const FusedFinish<PLAIN> fin) {
+    constexpr u32 HALF = (u32)PartCfg<WORDS>::HALF;
+    __shared__ u32 warp_tot[RADIX / 32];
+    if (blockIdx.x >= seg_num_tiles(sl)) return;
+    const uint4 t = __ldg(&sl.tiles[blockIdx.x]);
+    const u32 len = t.y, row = t.z, idx = t.w & 0xfffffu, seg = t.w >> 20;
+    const u32 d = threadIdx.x, lane = d & 31;
+    const u32 incl = __ldg(&status[(size_t)row * RADIX + d]) & VALUE_MASK;
+    const u32 excl = idx > 0 ? __ldg(&status[(size_t)(row - 1) * RADIX + d]) & VALUE_MASK : 0u;
+    const u32 cnt = incl - excl;
+    const u32 p = __ldg(&sl.segbase[(size_t)seg * RADIX + d]) + excl;       // output position of the tile's run of d
+    // tile-local start of the run: exclusive scan of the counts over the digits
+    u32 sc = cnt;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const u32 v = __shfl_up_sync(0xffffffffu, sc, o);
+        if (lane >= (u32)o) sc += v;
+    }
+    if (lane == 31) warp_tot[d >> 5] = sc;
+    __syncthreads();
+    u32 ls = sc - cnt;
+    for (u32 w = 0; w < (d >> 5); ++w) ls += warp_tot[w];
+    if (cnt > 0 && p > 0) fin.repair(out, n, p, claim);
+    if (len > HALF && ls < HALF && HALF < ls + cnt) fin.repair(out, n, p + (HALF - ls), claim);
+}
+
+bool fused_finish_enabled() {
+    static int on = -1;
+    if (on < 0) { const char* e = getenv("TG_FUSED_FINISH"); on = e ? atoi(e) : 1; }
+    return on != 0;
+}
+
 // digit passes of a key descriptor over the item's little-endian u64 words, least significant first
 int build_pass_list(const tg_key_desc* d, PassList* pl) {
     if (d->item_bytes != 8 && d->item_bytes != 16) return TG_ERR_ARG;
@@ -302,16 +498,49 @@ bool segmented_enabled() {
     return on != 0;
 }
 
+// The finishing pass of a prefix sort fused into its last prefix pass (FusedFinish): the key, the prefix, the flag that a group
+// was too long (device word, zeroed by run_segmented_passes).
+struct FinishArgs {
+    const tg_key_desc* desc;
+    bool plain_u64;
+    PrefixMask pm;
+    u32* fail;
+};
+
+// the last prefix pass with the fused finishing pass, then finish_repair_kernel (the attempt's one finishing launch)
+template <int WORDS, bool PLAIN>
+int launch_fused_last(tg_ctx* ctx, const FinishArgs& fa, const void* src, void* dst, u32 n, const RadixDigit& fn, u32* status,
+                      const SegList& sl) {
+    typedef typename ItemT<WORDS>::type Item;
+    FusedFinish<PLAIN> fin;
+    if (make_key_view(fa.desc, &fin.kv) != TG_OK) return tg_set_error(ctx, TG_ERR_ARG, "radix sort: unsupported key descriptor");
+    fin.pm = fa.pm;
+    fin.fail = fa.fail;
+    u32* claim;
+    const size_t claim_bytes = (((size_t)n + 31) / 32) * 4;
+    TG_TRY(tg_ws_get(ctx, WS_FINISH, claim_bytes, (void**)&claim));
+    TG_CUDA(ctx, cudaMemsetAsync(claim, 0, claim_bytes, ctx->stream));
+    TG_CUDA(ctx, cudaMemsetAsync(fa.fail, 0, 4, ctx->stream));
+    TG_TRY((launch_partition_v<WORDS, RadixDigit, true, false, false, FusedFinish<PLAIN>>(ctx, src, dst, n, fn, nullptr, status, sl,
+                                                                                        nullptr, fin)));
+    TG_LAUNCH_T(ctx, TG_K_FIXUP, (finish_repair_kernel<WORDS, PLAIN>), sl.num_tiles, RADIX, 0, (Item*)dst, n, sl, (const u32*)status,
+                claim, fin);
+    return TG_OK;
+}
+
 // `npos` stable passes (digit positions pos[0..npos), least significant first) inside the segments given by the
 // histogram of the digit the items are currently partitioned by (seg_size on the host, seg_start on the device)
 // first_unstable: the first of these passes orders by a digit below which nothing has been ordered yet, and the items are
 // nothing but their key: it may run with the cheaper unstable ranking.
 // seg_size == nullptr: the segment sizes are only known on the device (d_seg_size): the tile list is built there and nothing
 // waits for the host.
+// fin != nullptr: the last pass finishes the prefix sort (launch_fused_last); read fin->fail with finish_flag.
 template <int WORDS>
 int run_segmented_passes(tg_ctx* ctx, const PassList& pl, const int* pos, int npos, const u32* seg_size, const u32* d_seg_size,
-                         const u32* d_seg_start, size_t n, void** src, void** dst, bool first_unstable = false) {
+                         const u32* d_seg_start, size_t n, void** src, void** dst, bool first_unstable = false,
+                         const FinishArgs* fin = nullptr) {
     typedef typename ItemT<WORDS>::type Item;
+    if (fin && npos == 0) return tg_set_error(ctx, TG_ERR_ARG, "segmented passes: a fused finishing pass needs a pass");
     if (npos == 0) return TG_OK;
     if (npos > 4) return tg_set_error(ctx, TG_ERR_ARG, "segmented passes: at most 4 digit positions");
     // (pinned staging buffer 1: the chunk list of the pass before this may still be in flight from buffer 0; every caller
@@ -321,7 +550,7 @@ int run_segmented_passes(tg_ctx* ctx, const PassList& pl, const int* pos, int np
     const u32* d_total = nullptr;
     if (seg_size) TG_TRY(build_tile_list(ctx, RADIX, seg_size, tile_items<WORDS>(), 1, WS_SEG_TILES, &d_tiles, &total));
     else TG_TRY(build_seg_tiles_device(ctx, d_seg_size, d_seg_start, n, tile_items<WORDS>(), false, WS_SEG_TILES, &d_tiles, &d_total, &total));
-    if (total == 0) return TG_OK;
+    if (total == 0) return fin ? tg_set_error(ctx, TG_ERR_ARG, "segmented passes: a fused finishing pass needs items") : TG_OK;
     u32* tables;       // segcount [seg][npos][RADIX] | segbase [pos][seg][RADIX]
     const size_t table_words = (size_t)RADIX * npos * RADIX;
     TG_TRY(tg_ws_get(ctx, WS_SEG_TABLES, 2 * table_words * 4, (void**)&tables));
@@ -346,11 +575,35 @@ int run_segmented_passes(tg_ctx* ctx, const PassList& pl, const int* pos, int np
         sl.segbase = segbase + (size_t)i * RADIX * RADIX;
         if (i == 0 && first_unstable)
             TG_TRY((launch_partition_seg_unstable<WORDS, RadixDigit>(ctx, *src, *dst, (u32)n, fn, status + (size_t)i * pass_status_words, sl)));
+        else if (fin && i == npos - 1) {
+            if constexpr (WORDS == 1) {
+                if (fin->plain_u64 && !fin->desc->descending)
+                    TG_TRY((launch_fused_last<WORDS, true>(ctx, *fin, *src, *dst, (u32)n, fn, status + (size_t)i * pass_status_words, sl)));
+                else
+                    TG_TRY((launch_fused_last<WORDS, false>(ctx, *fin, *src, *dst, (u32)n, fn, status + (size_t)i * pass_status_words, sl)));
+            }
+            else TG_TRY((launch_fused_last<WORDS, false>(ctx, *fin, *src, *dst, (u32)n, fn, status + (size_t)i * pass_status_words, sl)));
+        }
         else
             TG_TRY((launch_partition_seg<WORDS, RadixDigit>(ctx, *src, *dst, (u32)n, fn, status + (size_t)i * pass_status_words, sl)));
         void* t = *src; *src = *dst; *dst = t;
     }
     return TG_OK;
+}
+
+// *ok = the finishing pass (separate or fused) found no group too long; synchronises the stream
+int finish_flag(tg_ctx* ctx, const u32* d_fail, bool* ok) {
+    u32* h_fail = (u32*)ctx->pinned + 7168;       // (byte offset 28 KB of the pinned scratch: the callers keep the histogram / OR-AND words at its start)
+    TG_CUDA(ctx, cudaMemcpyAsync(h_fail, d_fail, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    *ok = *h_fail == 0;
+    return TG_OK;
+}
+
+// After the finishing pass: *src = the sorted items if `sorted`; otherwise a permutation of the input stably ordered by the
+// prefix, what the general path expects: the last prefix pass's input after a fused finishing pass, its output otherwise.
+inline void finish_swap(bool fused, bool sorted, void** src, void** dst) {
+    if (sorted != fused) std::swap(*src, *dst);
 }
 
 // finishing pass of the prefix sort over src -> dst; *ok = no group was too long
@@ -366,11 +619,7 @@ int run_fixup(tg_ctx* ctx, const tg_key_desc* desc, bool plain_u64, const Prefix
         TG_LAUNCH_T(ctx, TG_K_FIXUP, (prefix_fixup_kernel<WORDS, true>), grid, FIX_THREADS, 0, (const Item*)src, (Item*)dst, (u32)n, kv, pm, d_fail);
     else
         TG_LAUNCH_T(ctx, TG_K_FIXUP, (prefix_fixup_kernel<WORDS, false>), grid, FIX_THREADS, 0, (const Item*)src, (Item*)dst, (u32)n, kv, pm, d_fail);
-    u32* h_fail = (u32*)ctx->pinned + 7168;       // (byte offset 28 KB of the pinned scratch: the callers keep the histogram / OR-AND words at its start)
-    TG_CUDA(ctx, cudaMemcpyAsync(h_fail, d_fail, 4, cudaMemcpyDeviceToHost, ctx->stream));
-    TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    *ok = *h_fail == 0;
-    return TG_OK;
+    return finish_flag(ctx, d_fail, ok);
 }
 
 // Speculative fast path of the prefix sort: assumes the position of the most significant varying key bit (ctx->spec_top_bit for
@@ -442,6 +691,7 @@ int prefix_sort_fast(tg_ctx* ctx, const tg_key_desc* desc, const PassList& pl, b
     static const bool unstable_ok = !(getenv("TG_UNSTABLE_RANK") && atoi(getenv("TG_UNSTABLE_RANK")) == 0);
     const bool key_only = unstable_ok && desc->key_bytes == desc->item_bytes && desc->key_offset == 0;
     static const bool optimistic = !(getenv("TG_SORT_OPTIMISTIC") && atoi(getenv("TG_SORT_OPTIMISTIC")) == 0);
+    const bool fused = fused_finish_enabled();
     if (bitwise && optimistic) {
         // Integer keys: the digits are fixed by the assumed top bit, so everything can be queued without waiting for the histogram
         // — the pass on the top digit, the tile list of its buckets (built on the device), the passes inside them, the finishing
@@ -458,9 +708,11 @@ int prefix_sort_fast(tg_ctx* ctx, const tg_key_desc* desc, const PassList& pl, b
             else TG_TRY((launch_partition_seg<WORDS, RadixDigit>(ctx, *src, *dst, (u32)n, top_fn, cstatus, sl)));
             void* t = *src; *src = *dst; *dst = t;
         }
-        TG_TRY((run_segmented_passes<WORDS>(ctx, pp, ppos, K - 1, nullptr, totals, gbase_top, n, src, dst, key_only)));
+        const FinishArgs fa = { desc, plain_u64, pmo, fail };
+        TG_TRY((run_segmented_passes<WORDS>(ctx, pp, ppos, K - 1, nullptr, totals, gbase_top, n, src, dst, key_only, fused ? &fa : nullptr)));
         bool ok = false;
-        TG_TRY((run_fixup<WORDS>(ctx, desc, plain_u64, pmo, *src, *dst, n, fail, &ok)));          // (the one synchronisation)
+        if (fused) TG_TRY(finish_flag(ctx, fail, &ok));                                           // (the one synchronisation)
+        else TG_TRY((run_fixup<WORDS>(ctx, desc, plain_u64, pmo, *src, *dst, n, fail, &ok)));
         int nonempty_o = 0;
         for (int d = 0; d < RADIX; ++d) nonempty_o += h_totals[d] ? 1 : 0;
         const int w = pp.word[0];
@@ -469,12 +721,11 @@ int prefix_sort_fast(tg_ctx* ctx, const tg_key_desc* desc, const PassList& pl, b
         if (tb_act != tb) ctx->spec_top_bit = tb_act > 8 ? tb_act : 8;           // what the next sort on this ctx should assume
         if (tb_act > tb || nonempty_o < 32) {
             if (tb_act <= tb && (tb_act + 7) / 8 < K + 2) ctx->prefix_spec_penalty = 8;
+            finish_swap(fused, false, src, dst);
             return TG_OK;                                                         // (*src: a permutation of the input)
         }
-        if (ok) {
-            void* t = *src; *src = *dst; *dst = t;
-            *taken = true;
-        }
+        finish_swap(fused, ok, src, dst);
+        if (ok) *taken = true;
         else {
             ctx->prefix_sort_penalty = 8;
             ctx->prefix_sort_fallbacks++;
@@ -522,15 +773,15 @@ int prefix_sort_fast(tg_ctx* ctx, const tg_key_desc* desc, const PassList& pl, b
         else TG_TRY((launch_partition_seg<WORDS, RadixDigit>(ctx, *src, *dst, (u32)n, top_fn, cstatus, sl)));
         void* t = *src; *src = *dst; *dst = t;
     }
-    // (2) the other K-1 prefix digits inside the buckets of (1)
-    TG_TRY((run_segmented_passes<WORDS>(ctx, pp, prefix_pos, K - 1, h_totals, nullptr, gbase_top, n, src, dst, key_only)));
-    // (3) finishing pass
+    // (2) the other K-1 prefix digits inside the buckets of (1), the last one with the finishing pass fused in
+    const FinishArgs fa = { desc, plain_u64, pm, fail };
+    TG_TRY((run_segmented_passes<WORDS>(ctx, pp, prefix_pos, K - 1, h_totals, nullptr, gbase_top, n, src, dst, key_only, fused ? &fa : nullptr)));
+    // (3) finishing pass (separate, or the fused pass's flag)
     bool ok = false;
-    TG_TRY((run_fixup<WORDS>(ctx, desc, plain_u64, pm, *src, *dst, n, fail, &ok)));
-    if (ok) {
-        void* t = *src; *src = *dst; *dst = t;
-        *taken = true;
-    }
+    if (fused) TG_TRY(finish_flag(ctx, fail, &ok));
+    else TG_TRY((run_fixup<WORDS>(ctx, desc, plain_u64, pm, *src, *dst, n, fail, &ok)));
+    finish_swap(fused, ok, src, dst);
+    if (ok) *taken = true;
     else {
         ctx->prefix_sort_penalty = 8;
         ctx->prefix_sort_fallbacks++;
@@ -602,20 +853,24 @@ int radix_sort_impl(tg_ctx* ctx, const tg_key_desc* desc, const PassList& pl, vo
         const int top = active[nactive - 1];
         int nonempty = 0;
         for (int d = 0; d < RADIX; ++d) nonempty += h_hist[top * RADIX + d] ? 1 : 0;
+        const PrefixMask pm = prefix_mask(desc, active[nactive - K]);
+        bool fused = false;
         if (segmented_enabled() && K >= 2 && nonempty >= 32) {
-            // most significant digit first (global pass), then the other K-1 digits inside its buckets
+            // most significant digit first (global pass), then the other K-1 digits inside its buckets, the last one with the
+            // finishing pass fused in
+            fused = fused_finish_enabled();
+            const FinishArgs fa = { desc, plain_u64, pm, fail };
             TG_TRY(run_pass(top));
             TG_TRY((run_segmented_passes<WORDS>(ctx, pl, active + (nactive - K), K - 1, h_hist + top * RADIX, nullptr,
-                                                 gbase + (size_t)top * RADIX, n, &src, &dst)));
+                                                 gbase + (size_t)top * RADIX, n, &src, &dst, false, fused ? &fa : nullptr)));
         }
         else
             for (int a = nactive - K; a < nactive; ++a) TG_TRY(run_pass(active[a]));
         bool ok = false;
-        TG_TRY((run_fixup<WORDS>(ctx, desc, plain_u64, prefix_mask(desc, active[nactive - K]), src, dst, n, fail, &ok)));
-        if (ok) {
-            void* t = src; src = dst; dst = t;
-            done = true;
-        }
+        if (fused) TG_TRY(finish_flag(ctx, fail, &ok));
+        else TG_TRY((run_fixup<WORDS>(ctx, desc, plain_u64, pm, src, dst, n, fail, &ok)));
+        finish_swap(fused, ok, &src, &dst);
+        if (ok) done = true;
         else {
             // a group of equal prefixes was longer than the finishing pass can see (heavy duplicates / clustered
             // keys): plain LSD over all active digits from the current permutation of the input; skip the attempt
