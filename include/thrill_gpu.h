@@ -22,7 +22,9 @@
  * indices of the result.  Merge (tg_merge and its forms) takes at most 2^30 - 1 items in a worker's k inputs together, and gives
  * each worker at most 2^30 - 1 items of the result; it merges 2..16 inputs of 8- or 16-byte items.  InnerJoin (tg_inner_join,
  * tg_inner_join_records and their _file forms) takes at most 2^30 - 1 items per worker and side, before and after its exchange, and gives each worker at
- * most 2^30 - 1 items of the result.  GroupByKey and GroupToIndex (tg_group_by_key, tg_group_to_index and their _file forms)
+ * most 2^30 - 1 items of the result.  ReduceByKey on records (tg_reduce_by_key_records and its _file form) takes at most 2^30 - 1
+ * items per worker, before and after its exchange; it reduces 4..1024-byte records by a 1..8-byte key field with at most 8 field
+ * runs.  GroupByKey and GroupToIndex (tg_group_by_key, tg_group_to_index and their _file forms)
  * take at most 2^30 - 1 items per worker, before and after their exchange.
  * PrefixSum, ExPrefixSum and ZipWithIndex (tg_prefix_sum, tg_zip_with_index, their _file and _select forms, tg_scan_local_total)
  * take at most 2^30 - 1 items per worker and give each worker as many items as it holds.  Sum, Min, Max and AllReduce (tg_all_reduce
@@ -135,7 +137,8 @@ enum { TG_K_RADIX_HIST = 0, TG_K_PARTITION = 1, TG_K_MERGE = 2, TG_K_PREAGG = 3,
        TG_K_HLL = 12 /* HyperLogLog's hash-and-register kernel (and the register merge of tg_hyperloglog_select) */,
        TG_K_WINDOW = 13 /* Window's block-fold kernel */,
        TG_K_SAMPLE = 14 /* Sample's and BernoulliSample's histogram, candidate, digit-pick, count, tile-scan and write kernels */,
-       TG_K_NUM = 15 };
+       TG_K_REDUCE_RECORDS = 15 /* ReduceByKey on records: the head count, tile scan, segmented field reduce and cut-group fold */,
+       TG_K_NUM = 16 };
 int tg_profile_enable(tg_ctx* ctx, int on);
 int tg_profile_get(tg_ctx* ctx, int kernel_class, float* out_total_ms, uint64_t* out_launches);
 /* the individual launch durations of `kernel_class` in launch order (up to `capacity`); *out_n = how many there are */
@@ -435,6 +438,59 @@ int tg_inner_join_records_file(tg_ctx* ctx, const tg_join_records_desc* desc, co
 int tg_exchange_records_select(tg_ctx* ctx, uint32_t mode, uint32_t item_bytes, uint32_t key_offset, uint32_t key_bytes,
                                const void* const* d_shards, const size_t* n_shards, uint32_t p, void* const* d_windows,
                                const size_t* window_bytes, uint64_t* out_counts);
+
+/* ---- ReduceByKey on records: DIA<T> of fixed-size PODs reduced by an unsigned integer key field, field by field
+ * (api::ReduceByKey, api/reduce_by_key.hpp:312-363; ReduceNode :100-211) -----------------------------------------------------------
+ * Items: a trivially copyable T serialized as its raw sizeof(T) bytes, or a pair<uint64_t, V> with V POD (8 + sizeof(V) bytes);
+ * 4 <= item_bytes <= 1024, a multiple of 4, records 4-byte aligned.  Key: an unsigned little-endian integer of key_bytes = 1..8
+ * bytes at byte offset key_offset (no alignment needed), compared zero-extended, as in tg_inner_join_records.
+ * The reduce function (thrill_gpu::FieldReduce<T>) is given as at most 8 field runs: run {offset, count, op} is `count`
+ * consecutive 8-byte fields from byte `offset` (a multiple of 4), each folded by op, one of TG_OP_SUM_F64, TG_OP_SUM_U64,
+ * TG_OP_MIN_U64, TG_OP_MAX_U64, TG_OP_MIN_F64, TG_OP_MAX_F64.  Runs lie inside the item and overlap neither each other nor the key
+ * bytes.  No runs keeps one item per key.
+ * Output: one item per distinct key.  Each run's fields hold the fold of the group's values; every other byte (the key, padding,
+ * fields no run names) comes from the group's item that is first in global input order (global position = position in the
+ * concatenation of the workers' shards).  The stock fold of FieldReduce<T> at p = 1 (a left fold in input order that keeps a's
+ * bytes, while its table does not spill) gives the same bytes; at p > 1 this is one of the outcomes the stock operator allows.
+ * Per field: integer ops are exact (sums wrap modulo 2^64); MIN/MAX_F64 give one of the group's own bit patterns, numerically the
+ * min/max of its non-NaN values (a NaN only where every value is a NaN; of equal values the earliest); double sums follow IEEE for
+ * NaN and inf, and a zero sum is -0.0 exactly when every value is -0.0.  Double sums are bracketed by positions and fixed tile
+ * sizes only (no atomics), so the same input on the same number of workers gives the same bytes.  Let exact be the exact sum of
+ * a group's values, A the same sum over |x|, u = 2^-53 and gamma_D = D u / (1 - D u), D the longest chain of additions a summand
+ * goes through in one local reduce of n records:
+ *   D = 32 + ceil(t / 256),  t = ceil(n / T) tiles, T = min(2048, 2^floor(log2(4096 / F))) for F fields in all runs
+ * (at most 23 inside a tile: a sequential fold of at most 16 items, at most 8 scan levels, one combine; then a thread's run of
+ * pieces, 8 tree levels and one combine for a group cut by tile edges).  With p > 1 a value goes through two local reduces (the
+ * pre phase on its worker, then its owner's reduce of what it receives), so D is the sum of the two.  While
+ * (1 + gamma_D) A < DBL_MAX, |out - exact| <= gamma_D A + u |exact|.  A NaN's payload is left open for sums.
+ * Placement and order: worker Hash128to64(0, key) % p owns a key, as in tg_reduce_by_key and the joins; a worker's result is in
+ * ascending key order (the stock node emits its table's order, so comparisons with it are on the multiset).
+ * Limits: 2^30 or more items on a worker, before or after the exchange, is TG_ERR_TOO_LARGE on every rank or on none.
+ * TG_ERR_ARG: a bad item size or key (as in tg_inner_join_records), more than 8 runs, a run with count 0, an op outside the six,
+ * an offset not a multiple of 4, a run outside the item or overlapping another run or the key, records not 4-byte aligned, a
+ * host File whose byte count is not a multiple of item_bytes, a device File whose item_bytes differs from the descriptor.
+ * Inputs are read, never modified; an input may be the un-detached result of an earlier operator on this ctx (one this operator
+ * would overwrite is copied out of the way first).  One local reduce: tuples {key, position} stably sorted by the key, a head
+ * count per tile and its scan, a segmented field reduce per tile that gathers only the run words, and one fold per group cut by
+ * tile edges (tg_reduce_records.cu).  With p > 1: the local reduce (the pre phase), the owner partition of its result, the
+ * count matrix, the records into the owners' windows, the local reduce of the received records.  Host round trips: with p = 1
+ * one (the output count; none for an empty input), with p > 1 three (the pre phase's output count, the count matrix, the output
+ * count).  Collective. */
+typedef struct {
+    uint32_t offset;           /* byte offset of the first field, a multiple of 4 */
+    uint32_t count;            /* consecutive 8-byte fields, >= 1 */
+    uint32_t op;               /* TG_OP_SUM_F64 .. TG_OP_MAX_F64 */
+} tg_field_run;
+typedef struct {
+    uint32_t item_bytes, key_offset, key_bytes, nruns;
+    tg_field_run runs[8];
+} tg_reduce_records_desc;
+/* device buffer; *out_dptr holds *out_n items of item_bytes, as for tg_sort (ctx-owned, valid until the next operator call) */
+int tg_reduce_by_key_records(tg_ctx* ctx, const tg_reduce_records_desc* desc, const void* d_in, size_t n_local, void** out_dptr,
+                             size_t* out_n);
+/* the drop-in call (GpuReduceNode<..., tg_reduce_records_desc>): a host File (Blocks) or a device File (read in place, left
+ * intact); the result is fetched with tg_fetch_output or taken with tg_output_detach */
+int tg_reduce_by_key_records_file(tg_ctx* ctx, const tg_reduce_records_desc* desc, const tg_merge_input* in, size_t* out_items);
 
 /* ---- GroupByKey / GroupToIndex: a DIA<pair<u64, V>> grouped by .first (DIA::GroupByKey, api/group_by_key.hpp:46-428;
  * DIA::GroupToIndex, api/group_to_index.hpp:36-290) ---------------------------------------------------------------------------

@@ -5,7 +5,8 @@ Mirrors (same names, argument meaning and error behaviour) the slice of thrill/a
     api::Generate(ctx, n, fn)              thrill/api/generate.hpp         (even range split over workers)
     DIA<T>::Sort(cmp) / SortStable(cmp)    thrill/api/sort.hpp:800-937
     DIA<T>::ReducePair(reduce_fn)          thrill/api/reduce_by_key.hpp:410-449
-    DIA<T>::ReduceByKey(key_ex, reduce_fn) thrill/api/reduce_by_key.hpp:312-363
+    DIA<T>::ReduceByKey(key_ex, reduce_fn) thrill/api/reduce_by_key.hpp:312-363 (pairs on .first; records on a KeyField with a
+                                           FieldReduce)
     DIA<T>::Merge(second, cmp) / api::Merge thrill/api/merge.hpp:674-721
     DIA<T>::GroupByKey / GroupToIndex      thrill/api/group_by_key.hpp:419-428, group_to_index.hpp:257-290
     DIA<T>::PrefixSum / ExPrefixSum        thrill/api/dia.hpp:1850, :1867 (api/prefix_sum.hpp, ex_prefix_sum.hpp)
@@ -69,6 +70,19 @@ def KeyField(offset, nbytes):
     byte offset `offset` of an item, zero-extended to uint64_t"""
     f = _Functor("KeyField<%d, %d>" % (offset, nbytes))
     f.key_offset, f.key_bytes = int(offset), int(nbytes)
+    return f
+
+
+def FieldReduce(runs):
+    """thrill_gpu::FieldReduce: the reduce function of ReduceByKey on records, given as at most 8 field runs (offset, count, f):
+    `count` consecutive 8-byte fields from byte `offset` (a multiple of 4), each folded by f, one of PlusDouble, PlusU64, MinU64,
+    MaxU64, MinDouble, MaxDouble.  Every other byte of a result comes from the group's first item.  No runs keeps one item per key."""
+    runs = [tuple(r) for r in runs]
+    for r in runs:
+        if len(r) != 3 or not isinstance(r[2], _Functor) or r[2].code is None or r[2] is First:
+            raise capi.ThrillGpuError("FieldReduce: run %r is not (offset, count, reduce function)" % (r,))
+    f = _Functor("FieldReduce<%s>" % ", ".join("{%d, %d, %s}" % (o, c, fn.name) for o, c, fn in runs))
+    f.runs = [(int(o), int(c), fn.code) for o, c, fn in runs]
     return f
 
 
@@ -239,13 +253,13 @@ def InnerJoin(first, second, key_extractor1, key_extractor2, join_function, **kw
     return DIA(first.ctx, first._fetch(n_out.value, dtype, dtype.itemsize, kw.get("_pinned_out")))
 
 
-def _record_bytes(items):
+def _record_bytes(items, what="InnerJoin: JoinPair"):
     """item size of a DIA of records: np.void or structured items, or rows of a 2-D uint8 array"""
     if items.ndim == 1 and items.dtype.kind == "V":
         return items.dtype.itemsize
     if items.ndim == 2 and items.dtype == np.uint8:
         return items.shape[1]
-    raise capi.ThrillGpuError("InnerJoin: JoinPair takes DIAs of np.void or structured items, not %r/%r" % (items.dtype, items.shape))
+    raise capi.ThrillGpuError("%s takes DIAs of np.void or structured items, not %r/%r" % (what, items.dtype, items.shape))
 
 
 def _inner_join_records(first, second, key1, key2, pinned_out):
@@ -505,10 +519,35 @@ class DIA(object):
         tg.ck(tg.L.tg_zip_with_index_file(tg.h, C.byref(inp), int(zip_function is IndexFirst), C.byref(n_out)))
         return DIA(self.ctx, self._fetch(n_out.value, KV, 16))
 
-    def ReduceByKey(self, key_extractor, reduce_function):
+    def ReduceByKey(self, key_extractor, reduce_function, _pinned_out=None):
+        """pair<uint64_t, 8-byte value> items with KeyIsFirst and a ReducePair function; or fixed-size records (np.void or structured
+        items, or rows of a 2-D uint8 array: 4..1024 bytes in multiples of 4) with KeyField(offset, nbytes) (KeyIsFirst for pair items)
+        and FieldReduce(runs).  Records: worker Hash128to64(0, key) % p holds a key's result, in ascending key order."""
+        if getattr(reduce_function, "runs", None) is not None:
+            return self._reduce_records(key_extractor, reduce_function, _pinned_out)
         if key_extractor is not KeyIsFirst:
             raise capi.ThrillGpuError("ReduceByKey: only the pair.first key extractor is recognised by the GPU path")
         return self.ReducePair(reduce_function)
+
+    def _reduce_records(self, key_extractor, reduce_function, pinned_out):
+        if key_extractor is KeyIsFirst:
+            key = (0, 8)                                 # pair<uint64_t, V>: .first is the first 8 bytes
+        elif getattr(key_extractor, "key_bytes", None) is not None:
+            key = (key_extractor.key_offset, key_extractor.key_bytes)
+        else:
+            raise capi.ThrillGpuError("ReduceByKey: FieldReduce takes KeyField or pair.first key extractors, not %r" % (key_extractor,))
+        it = self.items
+        ib = _record_bytes(it, "ReduceByKey: FieldReduce")
+        if len(reduce_function.runs) > 8:
+            raise capi.ThrillGpuError("ReduceByKey: at most 8 field runs")
+        desc = capi.reduce_records_desc(ib, key[0], key[1], reduce_function.runs)
+        blocks, nb = self._blocks(it)
+        inp = capi.MergeInput(None, C.cast(blocks, C.POINTER(capi.Block)), nb)
+        n_out = C.c_size_t()
+        tg = self.ctx.tg
+        tg.ck(tg.L.tg_reduce_by_key_records_file(tg.h, C.byref(desc), C.byref(inp), C.byref(n_out)))
+        out = self._fetch(n_out.value, None if it.ndim == 2 else it.dtype, ib, pinned_out)
+        return DIA(self.ctx, out)
 
     # ---- actions ---------------------------------------------------------------------------------------
     def _action_desc(self, what, fn):

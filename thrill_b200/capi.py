@@ -13,7 +13,7 @@ TG_OK = 0
 KEY_UINT_LE, KEY_BYTES_BE = 0, 1
 OP_SUM_F64, OP_SUM_U64, OP_MIN_U64, OP_MAX_U64, OP_MIN_F64, OP_MAX_F64, OP_FIRST = range(7)
 K_RADIX_HIST, K_PARTITION, K_MERGE, K_PREAGG, K_AGGREGATE, K_COMPACT, K_OTHER, K_FIXUP, K_SEGCOUNT, K_EXCHANGE, K_JOIN, K_SCAN, K_HLL, \
-    K_WINDOW, K_SAMPLE = range(15)
+    K_WINDOW, K_SAMPLE, K_REDUCE_RECORDS = range(16)
 WINDOW_FULL, WINDOW_PARTIAL, WINDOW_DISJOINT = range(3)
 JOIN_KEY_VALUES, JOIN_VALUES = 0, 1
 ROUTE_HASH, ROUTE_MOD, ROUTE_RANGE, ROUTE_SPLITTERS = range(4)
@@ -48,6 +48,23 @@ class JoinDesc(C.Structure):
 class JoinRecordsDesc(C.Structure):
     _fields_ = [("left_bytes", C.c_uint32), ("right_bytes", C.c_uint32), ("left_key_offset", C.c_uint32),
                 ("left_key_bytes", C.c_uint32), ("right_key_offset", C.c_uint32), ("right_key_bytes", C.c_uint32)]
+
+
+class FieldRun(C.Structure):
+    _fields_ = [("offset", C.c_uint32), ("count", C.c_uint32), ("op", C.c_uint32)]
+
+
+class ReduceRecordsDesc(C.Structure):
+    _fields_ = [("item_bytes", C.c_uint32), ("key_offset", C.c_uint32), ("key_bytes", C.c_uint32), ("nruns", C.c_uint32),
+                ("runs", FieldRun * 8)]
+
+
+def reduce_records_desc(item_bytes, key_offset, key_bytes, runs):
+    """tg_reduce_records_desc from runs = [(offset, count, op), ...] (at most 8)"""
+    d = ReduceRecordsDesc(item_bytes, key_offset, key_bytes, len(runs))
+    for i, (off, cnt, op) in enumerate(runs):
+        d.runs[i] = FieldRun(off, cnt, op)
+    return d
 
 
 class ScanDesc(C.Structure):
@@ -136,6 +153,8 @@ SYMBOLS = [
     ("tg_inner_join_records", _i, [_vp, _P(JoinRecordsDesc), _vp, _sz, _vp, _sz, _P(_vp), _P(_sz)]),
     ("tg_inner_join_records_file", _i, [_vp, _P(JoinRecordsDesc), _P(MergeInput), _P(MergeInput), _P(_sz)]),
     ("tg_exchange_records_select", _i, [_vp, _u32, _u32, _u32, _u32, _P(_vp), _P(_sz), _u32, _P(_vp), _P(_sz), _P(_u64)]),
+    ("tg_reduce_by_key_records", _i, [_vp, _P(ReduceRecordsDesc), _vp, _sz, _P(_vp), _P(_sz)]),
+    ("tg_reduce_by_key_records_file", _i, [_vp, _P(ReduceRecordsDesc), _P(MergeInput), _P(_sz)]),
     ("tg_group_by_key", _i, [_vp, _vp, _sz, _P(_vp), _P(_sz)]),
     ("tg_group_to_index", _i, [_vp, _vp, _sz, _u64, _P(_vp), _P(_sz), _P(_u64), _P(_u64)]),
     ("tg_group_by_key_file", _i, [_vp, _P(MergeInput), _P(_sz)]),

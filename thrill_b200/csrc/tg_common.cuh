@@ -15,7 +15,7 @@
 typedef unsigned long long u64;
 typedef unsigned int u32;
 
-#define TG_NUM_WS 37
+#define TG_NUM_WS 41
 #define TG_MAX_RANKS 16
 
 struct tg_ctx {
@@ -84,7 +84,10 @@ enum { WS_SORT_TMP = 0, WS_SORT_STATUS = 1, WS_SORT_HIST = 2, WS_XCHG_SEND = 3, 
        // that lies in a slot the join writes (an un-detached join or GroupByKey result), copied out of the way (left, right)
        WS_JOIN_LREC = 33, WS_JOIN_IN_L = 34, WS_JOIN_IN_R = 35,
        // radix sort (tg_radix_sort.cu): one bit per item, the group heads claimed by the fused finishing pass's repair kernel
-       WS_FINISH = 36 };
+       WS_FINISH = 36,
+       // ReduceByKey on records (tg_reduce_records.cu): the sorted tuples (+ sort scratch); tile sums, bases and partials; the
+       // output (with p > 1 also the pre phase's); an input that lies in one of these slots, copied out of the way
+       WS_RR_TUP = 37, WS_RR_AUX = 38, WS_RR_OUT = 39, WS_RR_IN = 40 };
 
 int tg_set_error(tg_ctx* ctx, int status, const char* fmt, ...);
 int tg_ws_get(tg_ctx* ctx, int slot, size_t bytes, void** out);

@@ -20,6 +20,7 @@
 // worker's records then go through steps 2-5 as the pairs do, except that the emit (join_emit_records_kernel) writes each output
 // as the left record's words followed by the right record's, read where the records lie.
 #include <algorithm>
+#include <initializer_list>
 
 #include "tg_keys.cuh"
 #include "tg_exchange.cuh"
@@ -302,17 +303,6 @@ int join_impl(tg_ctx* ctx, const tg_join_desc* desc, const void* d_left, size_t 
 }
 
 // ---- records ----------------------------------------------------------------------------------------------------------------
-struct RecSide {
-    u32 bytes, key_off, key_bytes;
-};
-
-int check_side(tg_ctx* ctx, const char* what, const RecSide& s) {
-    if (s.bytes == 0 || s.bytes % 4 || s.bytes > 1024 || s.key_bytes == 0 || s.key_bytes > 8 || (u64)s.key_off + s.key_bytes > s.bytes)
-        return tg_set_error(ctx, TG_ERR_ARG, "%s: item size %u (a multiple of 4, 4..1024) with a key of %u bytes at offset %u (1..8 bytes "
-                            "inside the item)", what, s.bytes, s.key_bytes, s.key_off);
-    return TG_OK;
-}
-
 int check_join_records_args(tg_ctx* ctx, const tg_join_records_desc* d, RecSide* side) {
     if (!ctx || !d) return tg_set_error(ctx, TG_ERR_ARG, "inner_join_records: NULL argument");
     side[0] = { d->left_bytes, d->left_key_offset, d->left_key_bytes };
@@ -323,59 +313,16 @@ int check_join_records_args(tg_ctx* ctx, const tg_join_records_desc* d, RecSide*
     return TG_OK;
 }
 
-// the n records' tuples in workspace `slot` (tuples | sort scratch), stably sorted by the key: *sorted
-int sort_record_tuples(tg_ctx* ctx, int slot, const void* rec, u64 n, const RecSide& s, const Pair** sorted) {
-    Pair* buf;
-    TG_TRY(tg_ws_get(ctx, slot, (2 * n + 2) * 16, (void**)&buf));
-    *sorted = buf;
-    if (!n) return TG_OK;
-    TG_LAUNCH(ctx, make_tuples_kernel, ctx->sm_count * 8, 256, 0, (const u32*)rec, (u32)n, s.bytes / 4, s.key_off, s.key_bytes, buf);
-    const tg_key_desc sd = { 16, 0, 8, TG_KEY_UINT_LE, 0, 1 };
-    void* res = buf;
-    TG_TRY(tg_radix_sort_items(ctx, &sd, buf, buf + n + 1, n, &res));
-    *sorted = (const Pair*)res;
-    return TG_OK;
-}
-
-// worker w's n records: their tuples into tup, partitioned by the owner into ptup; *d_tot = the per-destination counts (device)
-int partition_record_tuples(tg_ctx* ctx, const void* rec, size_t n, const RecSide& s, u32 p, Pair** ptup, u32** d_tot) {
-    Pair* tup;
-    TG_TRY(tg_ws_get(ctx, WS_JOIN_L, (n + 1) * 16, (void**)&tup));
-    TG_TRY(tg_ws_get(ctx, WS_JOIN_R, (n + 1) * 16, (void**)ptup));
-    if (n) TG_LAUNCH(ctx, make_tuples_kernel, ctx->sm_count * 8, 256, 0, (const u32*)rec, (u32)n, s.bytes / 4, s.key_off, s.key_bytes, tup);
-    const HashDigit fn = { p };
-    return partition_chunked<2, HashDigit>(ctx, tup, *ptup, n, fn, d_tot, nullptr);
-}
-
-// An input that lies in a slot the join writes before its last read of the inputs (WS_JOIN_L / WS_JOIN_R: the tuples, and the
-// result of GroupByKey; WS_JOIN_OUT: the result of a join) is copied out of the way first, into WS_JOIN_IN_L / WS_JOIN_IN_R.  The
-// two sides of a self-join stay one copy.
-int move_inputs_out_of_join_slots(tg_ctx* ctx, const void** rec, const size_t* bytes) {
-    const void* orig[2] = { rec[0], rec[1] };
-    for (int j = 0; j < 2; ++j) {
-        const char* q = (const char*)orig[j];
-        bool inside = false;
-        for (const int s : { WS_JOIN_L, WS_JOIN_R, WS_JOIN_OUT }) {
-            const char* b = (const char*)ctx->ws[s];
-            if (bytes[j] && b && q >= b && q < b + ctx->ws_bytes[s]) inside = true;
-        }
-        if (!inside) continue;
-        if (j == 1 && orig[1] == orig[0] && bytes[1] == bytes[0]) { rec[1] = rec[0]; continue; }
-        void* d;
-        TG_TRY(tg_ws_get(ctx, j ? WS_JOIN_IN_R : WS_JOIN_IN_L, bytes[j], &d));
-        TG_CUDA(ctx, cudaMemcpyAsync(d, q, bytes[j], cudaMemcpyDeviceToDevice, ctx->stream));
-        rec[j] = d;
-    }
-    return TG_OK;
-}
-
 int join_records_impl(tg_ctx* ctx, const RecSide* side, const void* d_left, size_t n_left, const void* d_right, size_t n_right,
                       void** out_dptr, size_t* out_n) {
     const int p = ctx->nranks;
     const void* rec[2] = { d_left, d_right };
     u64 n[2] = { n_left, n_right };
     const size_t bytes[2] = { n_left < JOIN_LIMIT ? n_left * side[0].bytes : 0, n_right < JOIN_LIMIT ? n_right * side[1].bytes : 0 };
-    TG_TRY(move_inputs_out_of_join_slots(ctx, rec, bytes));
+    // an input in a slot the join writes before its last read of the inputs (WS_JOIN_L / WS_JOIN_R: the tuples, and the result of
+    // GroupByKey; WS_JOIN_OUT: the result of a join) is copied out of the way first; the two sides of a self-join stay one copy
+    const int dst[2] = { WS_JOIN_IN_L, WS_JOIN_IN_R };
+    TG_TRY(move_inputs_out_of_slots(ctx, rec, bytes, 2, { WS_JOIN_L, WS_JOIN_R, WS_JOIN_OUT }, dst));
     if (p == 1) {
         if (n_left >= JOIN_LIMIT || n_right >= JOIN_LIMIT)
             return tg_set_error(ctx, TG_ERR_TOO_LARGE, "inner_join_records: %zu x %zu items (limit 2^30 - 1 per side)", n_left, n_right);
@@ -430,6 +377,63 @@ int join_records_impl(tg_ctx* ctx, const RecSide* side, const void* d_left, size
 }
 
 }  // namespace
+
+namespace tgp {
+
+int check_side(tg_ctx* ctx, const char* what, const RecSide& s) {
+    if (s.bytes == 0 || s.bytes % 4 || s.bytes > 1024 || s.key_bytes == 0 || s.key_bytes > 8 || (u64)s.key_off + s.key_bytes > s.bytes)
+        return tg_set_error(ctx, TG_ERR_ARG, "%s: item size %u (a multiple of 4, 4..1024) with a key of %u bytes at offset %u (1..8 bytes "
+                            "inside the item)", what, s.bytes, s.key_bytes, s.key_off);
+    return TG_OK;
+}
+
+// the n records' tuples in workspace `slot` (tuples | sort scratch), stably sorted by the key: *sorted
+int sort_record_tuples(tg_ctx* ctx, int slot, const void* rec, u64 n, const RecSide& s, const Pair** sorted) {
+    Pair* buf;
+    TG_TRY(tg_ws_get(ctx, slot, (2 * n + 2) * 16, (void**)&buf));
+    *sorted = buf;
+    if (!n) return TG_OK;
+    TG_LAUNCH(ctx, make_tuples_kernel, ctx->sm_count * 8, 256, 0, (const u32*)rec, (u32)n, s.bytes / 4, s.key_off, s.key_bytes, buf);
+    const tg_key_desc sd = { 16, 0, 8, TG_KEY_UINT_LE, 0, 1 };
+    void* res = buf;
+    TG_TRY(tg_radix_sort_items(ctx, &sd, buf, buf + n + 1, n, &res));
+    *sorted = (const Pair*)res;
+    return TG_OK;
+}
+
+// worker w's n records: their tuples into tup, partitioned by the owner into ptup; *d_tot = the per-destination counts (device)
+int partition_record_tuples(tg_ctx* ctx, const void* rec, size_t n, const RecSide& s, u32 p, Pair** ptup, u32** d_tot) {
+    Pair* tup;
+    TG_TRY(tg_ws_get(ctx, WS_JOIN_L, (n + 1) * 16, (void**)&tup));
+    TG_TRY(tg_ws_get(ctx, WS_JOIN_R, (n + 1) * 16, (void**)ptup));
+    if (n) TG_LAUNCH(ctx, make_tuples_kernel, ctx->sm_count * 8, 256, 0, (const u32*)rec, (u32)n, s.bytes / 4, s.key_off, s.key_bytes, tup);
+    const HashDigit fn = { p };
+    return partition_chunked<2, HashDigit>(ctx, tup, *ptup, n, fn, d_tot, nullptr);
+}
+
+// An input that lies in one of `slots` is copied out of the way first, input j into dst_slots[j].  Inputs that are the same span
+// as input 0 stay one copy.
+int move_inputs_out_of_slots(tg_ctx* ctx, const void** rec, const size_t* bytes, int k, std::initializer_list<int> slots,
+                             const int* dst_slots) {
+    const void* orig0 = rec[0];
+    for (int j = 0; j < k; ++j) {
+        const char* q = (const char*)rec[j];
+        bool inside = false;
+        for (const int s : slots) {
+            const char* b = (const char*)ctx->ws[s];
+            if (bytes[j] && b && q >= b && q < b + ctx->ws_bytes[s]) inside = true;
+        }
+        if (!inside) continue;
+        if (j > 0 && rec[j] == orig0 && bytes[j] == bytes[0]) { rec[j] = rec[0]; continue; }
+        void* d;
+        TG_TRY(tg_ws_get(ctx, dst_slots[j], bytes[j], &d));
+        TG_CUDA(ctx, cudaMemcpyAsync(d, q, bytes[j], cudaMemcpyDeviceToDevice, ctx->stream));
+        rec[j] = d;
+    }
+    return TG_OK;
+}
+
+}  // namespace tgp
 
 extern "C" {
 

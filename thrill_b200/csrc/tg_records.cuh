@@ -1,6 +1,9 @@
 // tg_records.cuh — fixed-size records handled through 16-byte tuples {key bytes, u32 position}: Sort's record path
-// (tg_sample_sort.cu) and InnerJoin on records (tg_join.cu).  Records are a multiple of 4 bytes long and 4-byte aligned.
+// (tg_sample_sort.cu), InnerJoin on records (tg_join.cu) and ReduceByKey on records (tg_reduce_records.cu).  Records are a
+// multiple of 4 bytes long and 4-byte aligned.
 #pragma once
+#include <initializer_list>
+
 #include "tg_common.cuh"
 
 namespace {
@@ -44,6 +47,27 @@ inline u32 gather_reciprocal(u32 rec_words) {
 }  // namespace
 
 namespace tgp {
+
+// a record type: item size, and its key field (an unsigned little-endian integer of key_bytes = 1..8 bytes at byte offset key_off)
+struct RecSide {
+    u32 bytes, key_off, key_bytes;
+};
+
+// TG_ERR_ARG unless the size is a multiple of 4 in 4..1024 and the key is 1..8 bytes inside the item (`what` heads the message)
+int check_side(tg_ctx* ctx, const char* what, const RecSide& s);
+
+// the n records' tuples in workspace `slot` (tuples | sort scratch), stably sorted by the key: *sorted  (tg_join.cu)
+int sort_record_tuples(tg_ctx* ctx, int slot, const void* rec, u64 n, const RecSide& s, const ulonglong2** sorted);
+
+// worker w's n records: their tuples into WS_JOIN_L, partitioned by the owner Hash128to64(0, key) % p into *ptup (WS_JOIN_R);
+// *d_tot = the per-destination counts (device)  (tg_join.cu)
+int partition_record_tuples(tg_ctx* ctx, const void* rec, size_t n, const RecSide& s, u32 p, ulonglong2** ptup, u32** d_tot);
+
+// An operator's k inputs (rec[j], bytes[j] bytes) that lie in a workspace slot it writes (`slots`: an un-detached result of an
+// earlier operator) are copied out of the way first, input j into dst_slots[j]; rec[j] is updated.  An input that is the same
+// span as input 0 stays one copy.  (tg_join.cu)
+int move_inputs_out_of_slots(tg_ctx* ctx, const void** rec, const size_t* bytes, int k, std::initializer_list<int> slots,
+                             const int* dst_slots);
 
 // Store step of the records' exchange for worker `me` of p: d_ptup = its n tuples partitioned by destination, counts = the p x p
 // count matrix (host), windows[d] = worker d's window.  Mode 1 stores the records straight into the windows, mode 0 into the

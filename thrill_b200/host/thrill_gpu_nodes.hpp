@@ -49,6 +49,7 @@
 #include <tlx/meta/vexpand.hpp>
 
 #include <array>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <functional>
@@ -265,15 +266,68 @@ struct JoinPair {
 //! with KeyFirst (8 + sizeof(V) bytes, serialized member-wise, the key first)
 template <typename T, typename KeyExtractor>
 struct RecordKey { static constexpr bool supported = false; };
+//! items written as their raw in-memory bytes: PODs, and std::pair<L, R> of two such items without padding (JoinPair's result)
+template <typename T>
+struct IsRawRecord : std::is_pod<T> { };
+template <typename L, typename R>
+struct IsRawRecord<std::pair<L, R> >
+    : std::integral_constant<bool, IsRawRecord<L>::value && IsRawRecord<R>::value && sizeof(std::pair<L, R>) == sizeof(L) + sizeof(R)> { };
 template <typename T>
 struct RecordKey<T, KeyField<T> >{
-    static constexpr bool supported = UintKeyTraits<T>::is_uint_key && std::is_pod<T>::value;
+    static constexpr bool supported = UintKeyTraits<T>::is_uint_key && IsRawRecord<T>::value;
     static constexpr uint32_t bytes = sizeof(T), key_offset = UintKeyTraits<T>::key_offset, key_bytes = UintKeyTraits<T>::key_bytes;
 };
 template <typename V>
 struct RecordKey<std::pair<uint64_t, V>, KeyFirst>{
     static constexpr bool supported = std::is_pod<V>::value;
     static constexpr uint32_t bytes = 8 + sizeof(V), key_offset = 0, key_bytes = 8;
+};
+
+//! ReduceByKey on records: name an item type's reduce function as field runs by specialising
+//!   template <> struct thrill_gpu::ReduceFieldsTraits<CC3> { static constexpr bool is_reduce_fields = true;
+//!       static std::vector<tg_field_run> runs() { return { { 8, 3, TG_OP_SUM_F64 }, { 32, 1, TG_OP_SUM_U64 } }; } };
+//! Run {offset, count, op}: count consecutive 8-byte fields from byte offset, each folded by op (TG_OP_SUM_F64 .. TG_OP_MAX_F64).
+//! FieldReduce<T> is the reduce function: a plain functor that folds b's run fields into a copy of a and keeps a's other bytes,
+//! so the stock dia.ReduceByKey(KeyField<T>(), FieldReduce<T>()) takes the same call.
+template <typename T>
+struct ReduceFieldsTraits {
+    static constexpr bool is_reduce_fields = false;
+};
+//! one 8-byte field folded as the library folds it (op_combine: of equal values the left one stays; a NaN only where both are)
+inline uint64_t FieldCombine(uint32_t op, uint64_t a, uint64_t b) {
+    double x, y, r;
+    std::memcpy(&x, &a, 8);
+    std::memcpy(&y, &b, 8);
+    switch (op) {
+    case TG_OP_SUM_F64: r = x + y; std::memcpy(&a, &r, 8); return a;
+    case TG_OP_SUM_U64: return a + b;
+    case TG_OP_MIN_U64: return b < a ? b : a;
+    case TG_OP_MAX_U64: return a < b ? b : a;
+    default: {               // TG_OP_MIN_F64 / TG_OP_MAX_F64
+        const bool better = (op == TG_OP_MIN_F64 ? y < x : x < y) ||
+                            (std::isnan(x) && (!std::isnan(y) || a == 0x7FF8000000000000ull));
+        return better ? b : a;
+    }
+    }
+}
+template <typename T>
+struct FieldReduce {
+    T operator () (const T& a, const T& b) const {
+        static_assert(ReduceFieldsTraits<T>::is_reduce_fields, "thrill_gpu::FieldReduce<T>: specialise thrill_gpu::ReduceFieldsTraits<T>");
+        T r = a;
+        char* pr = reinterpret_cast<char*>(&r);
+        const char* pb = reinterpret_cast<const char*>(&b);
+        for (const tg_field_run& run : ReduceFieldsTraits<T>::runs()) {
+            for (uint32_t j = 0; j < run.count; ++j) {
+                uint64_t x, y;
+                std::memcpy(&x, pr + run.offset + 8 * j, 8);
+                std::memcpy(&y, pb + run.offset + 8 * j, 8);
+                x = FieldCombine(run.op, x, y);
+                std::memcpy(pr + run.offset + 8 * j, &x, 8);
+            }
+        }
+        return r;
+    }
 };
 
 //! The sum function thrill_gpu::PrefixSum / ExPrefixSum recognise on pair<uint64_t, V>: F (one of the ReducePair functions,
@@ -540,7 +594,32 @@ private:
     bool have_host_file_ = false;
 };
 
-template <typename ValueType>
+//! ReduceNode's pre phase, exchange and post phase (api/reduce_by_key.hpp:100-211) behind the library: pairs (tg_kv_desc: ReducePair,
+//! ReduceByKey on KeyFirst / OnSecond, ReduceToIndex) or records (tg_reduce_records_desc: ReduceByKey on KeyField / FieldReduce)
+inline uint32_t ReduceItemBytes(const tg_kv_desc& d) { return d.item_bytes; }
+inline uint32_t ReduceItemBytes(const tg_reduce_records_desc& d) { return d.item_bytes; }
+inline void ReduceDev(tg_ctx* c, const tg_kv_desc& d, bool to_index, size_t size, const void* neutral, const tg_dev_file* in,
+                      size_t* out_items, uint64_t* begin) {
+    if (to_index) Check(c, tg_reduce_to_index_dev(c, &d, in, size, neutral, out_items, begin), "tg_reduce_to_index_dev");
+    else Check(c, tg_reduce_dev(c, &d, in, out_items), "tg_reduce_dev");
+}
+inline void ReduceDev(tg_ctx* c, const tg_reduce_records_desc& d, bool, size_t, const void*, const tg_dev_file* in,
+                      size_t* out_items, uint64_t*) {
+    const tg_merge_input mi { in, nullptr, 0 };
+    Check(c, tg_reduce_by_key_records_file(c, &d, &mi, out_items), "tg_reduce_by_key_records_file");
+}
+inline void ReduceHost(tg_ctx* c, const tg_kv_desc& d, bool to_index, size_t size, const void* neutral, const tg_block* blocks,
+                       size_t nblocks, size_t* out_items, uint64_t* begin) {
+    if (to_index) Check(c, tg_reduce_to_index_file(c, &d, blocks, nblocks, size, neutral, out_items, begin), "tg_reduce_to_index_file");
+    else Check(c, tg_reduce_file(c, &d, blocks, nblocks, out_items), "tg_reduce_file");
+}
+inline void ReduceHost(tg_ctx* c, const tg_reduce_records_desc& d, bool, size_t, const void*, const tg_block* blocks,
+                       size_t nblocks, size_t* out_items, uint64_t*) {
+    const tg_merge_input mi { nullptr, blocks, nblocks };
+    Check(c, tg_reduce_by_key_records_file(c, &d, &mi, out_items), "tg_reduce_by_key_records_file");
+}
+
+template <typename ValueType, typename Desc = tg_kv_desc>
 class GpuReduceNode final : public thrill::api::DOpNode<ValueType>, public GpuNodeBase
 {
     using Super = thrill::api::DOpNode<ValueType>;
@@ -548,13 +627,13 @@ class GpuReduceNode final : public thrill::api::DOpNode<ValueType>, public GpuNo
 
 public:
     template <typename ParentDIA>
-    GpuReduceNode(const ParentDIA& parent, const tg_kv_desc& desc)
+    GpuReduceNode(const ParentDIA& parent, const Desc& desc)
         : GpuReduceNode(parent, desc, false, 0, ValueType()) { }
 
     //! to_index: ReduceToIndexNode (api/reduce_to_index.hpp:60-237) — dense result of result_size items, neutral_element
     //! where no item has that index; worker r holds the index range Range(0, size).Partition(r, p)
     template <typename ParentDIA>
-    GpuReduceNode(const ParentDIA& parent, const tg_kv_desc& desc, bool to_index, size_t result_size,
+    GpuReduceNode(const ParentDIA& parent, const Desc& desc, bool to_index, size_t result_size,
                   const ValueType& neutral_element)
         : Super(parent.ctx(), to_index ? "GpuReduceToIndex" : "GpuReducePair", { parent.id() }, { parent.node() }),
           desc_(desc), parent_stack_empty_(ParentDIA::stack_empty),
@@ -577,7 +656,7 @@ public:
     }
 
     bool OnPreOpDeviceFile(const DeviceFilePtr& file, size_t item_bytes, size_t /* parent_index */) final {
-        if (!parent_stack_empty_ || item_bytes != sizeof(ValueType)) return false;
+        if (!parent_stack_empty_ || item_bytes != ReduceItemBytes(desc_)) return false;
         device_input_ = file;
         return true;
     }
@@ -588,23 +667,14 @@ public:
         input_writer_.Close();
         tg_ctx* c = WorkerCtx(context_);
         size_t out_items = 0;
-        static_assert(sizeof(ValueType) == 16, "16-byte (key, value) items");
         uint64_t begin = 0;
         if (device_input_) {
-            if (to_index_)
-                Check(c, tg_reduce_to_index_dev(c, &desc_, device_input_->get(), result_size_, &neutral_, &out_items, &begin),
-                      "tg_reduce_to_index_dev");
-            else
-                Check(c, tg_reduce_dev(c, &desc_, device_input_->get(), &out_items), "tg_reduce_dev");
+            ReduceDev(c, desc_, to_index_, result_size_, &neutral_, device_input_->get(), &out_items, &begin);
             device_input_.reset();
         }
         else {
             PinnedFileView view(input_file_, context_.local_worker_id());
-            if (to_index_)
-                Check(c, tg_reduce_to_index_file(c, &desc_, view.data(), view.size(), result_size_, &neutral_, &out_items, &begin),
-                      "tg_reduce_to_index_file");
-            else
-                Check(c, tg_reduce_file(c, &desc_, view.data(), view.size(), &out_items), "tg_reduce_file");
+            ReduceHost(c, desc_, to_index_, result_size_, &neutral_, view.data(), view.size(), &out_items, &begin);
         }
         input_file_.Clear();
         tg_dev_file f;
@@ -621,11 +691,11 @@ public:
         if (device_result_ && AllChildrenAreGpuNodes(*this)) {
             bool all = true;
             for (const auto& ch : this->children_)
-                all = dynamic_cast<GpuNodeBase*>(ch.node)->OnPreOpDeviceFile(device_result_, sizeof(ValueType), ch.parent_index) && all;
+                all = dynamic_cast<GpuNodeBase*>(ch.node)->OnPreOpDeviceFile(device_result_, ReduceItemBytes(desc_), ch.parent_index) && all;
             if (all) return;
         }
         if (!have_host_file_) {
-            FetchDeviceFileIntoFile(WorkerCtx(context_), context_, *device_result_, sizeof(ValueType), reduced_file_);
+            FetchDeviceFileIntoFile(WorkerCtx(context_), context_, *device_result_, ReduceItemBytes(desc_), reduced_file_);
             have_host_file_ = true;
         }
         this->PushFile(reduced_file_, consume);
@@ -634,7 +704,7 @@ public:
     void Dispose() final { reduced_file_.Clear(); device_result_.reset(); have_host_file_ = false; }
 
 private:
-    tg_kv_desc desc_;
+    Desc desc_;
     const bool parent_stack_empty_;
     const bool to_index_ = false;
     const size_t result_size_ = 0;
@@ -1484,6 +1554,38 @@ template <typename Key, typename Value, typename Stack, typename ValueFunction>
 auto ReduceByKey(const DIA<std::pair<Key, Value>, Stack>& dia, const KeyFirst& /* key_extractor */,
                  const OnSecond<ValueFunction>& reduce_function) {
     return ReducePair(dia, reduce_function.fn);
+}
+
+//! DIA<T>::ReduceByKey(key_extractor, reduce_function) on records: T a POD whose key field UintKeyTraits<T> names (KeyField<T>),
+//! or pair<uint64_t, V> with a POD V (KeyFirst), 4..1024 bytes in multiples of 4; reduce_function FieldReduce<T> with the runs of
+//! ReduceFieldsTraits<T>.  An output holds the folded fields and the other bytes of its key's first item in global input order;
+//! worker Hash128to64(0, key) % p holds a key, in ascending key order.  The result goes to GPU children as a device File.  Other
+//! item types or reduce functions: use the stock dia.ReduceByKey(key_extractor, reduce_function).
+template <typename ValueType, typename Stack, typename KeyExtractor>
+auto ReduceByKey(const DIA<ValueType, Stack>& dia, const KeyExtractor& /* key_extractor */,
+                 const FieldReduce<ValueType>& /* reduce_function */) {
+    using RK = RecordKey<ValueType, KeyExtractor>;
+    static_assert(RK::supported && ReduceFieldsTraits<ValueType>::is_reduce_fields,
+                  "thrill_gpu::ReduceByKey: records need a POD with KeyField<T> (UintKeyTraits) or pair<uint64_t, POD> with KeyFirst, "
+                  "and ReduceFieldsTraits<T>; use the stock dia.ReduceByKey(key_extractor, reduce_function)");
+    static_assert(RK::bytes % 4 == 0 && RK::bytes <= 1024 && RK::bytes == sizeof(ValueType),
+                  "thrill_gpu::ReduceByKey: records of 4..1024 bytes in multiples of 4, without padding; "
+                  "use the stock dia.ReduceByKey(key_extractor, reduce_function)");
+    static_assert(RK::key_bytes >= 1 && RK::key_bytes <= 8 && RK::key_offset + RK::key_bytes <= RK::bytes,
+                  "thrill_gpu::ReduceByKey: keys are unsigned integers of 1..8 bytes inside the item; "
+                  "use the stock dia.ReduceByKey(key_extractor, reduce_function)");
+    assert(dia.IsValid());
+    tg_reduce_records_desc d;
+    std::memset(&d, 0, sizeof(d));
+    d.item_bytes = RK::bytes;
+    d.key_offset = RK::key_offset;
+    d.key_bytes = RK::key_bytes;
+    const std::vector<tg_field_run> runs = ReduceFieldsTraits<ValueType>::runs();
+    if (runs.size() > 8) die("thrill_gpu::ReduceByKey: at most 8 field runs");
+    d.nruns = static_cast<uint32_t>(runs.size());
+    for (size_t i = 0; i < runs.size(); ++i) d.runs[i] = runs[i];
+    auto node = tlx::make_counting<GpuReduceNode<ValueType, tg_reduce_records_desc> >(dia, d);
+    return DIA<ValueType>(node);
 }
 
 //! DIA<pair<uint64_t index, V>>::ReduceToIndex(key = .first, reduce function on .second, size, neutral_element)
